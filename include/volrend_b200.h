@@ -238,6 +238,25 @@ unsigned long long vr_launch_count(void);
 const char* vr_last_error(void);
 const char* vr_version(void);
 
+/* ---- meshes (volrend_b200/csrc/vr_raster.cu) --------------------------------------------------------------
+ * The GL mesh pass of cuda_renderer.cpp:83-113 (Mesh::draw, src/mesh.cpp:98-160,366-396) as a CUDA rasterizer.
+ * A vertex is 9 floats: position, colour, normal (mesh.cpp:26).  face_size 3 / 2 / 1 = triangles / lines /
+ * points (4x4 pixels); with faces_dev NULL the primitives are consecutive vertices, n_verts / face_size of
+ * them, and n_faces is ignored.  A primitive with an index >= n_verts is not drawn.  unlit != 0 writes the
+ * vertex colour, otherwise the reference's fixed three-light Phong shader (mesh.cpp:137-156). */
+typedef struct {
+    const float* vert_dev;      /* n_verts * 9 floats, device (caller-owned, like every buffer here) */
+    const uint32_t* faces_dev;  /* n_faces * face_size indices, or NULL = consecutive vertices */
+    int32_t n_verts, n_faces, face_size, unlit;
+    float model[16];            /* column-major model matrix (host computes it from rotation/translation/scale) */
+} vr_mesh_desc;
+/* Draws meshes in order over the existing rgba8_dev (W*H*4) and depth_dev (W*H float, ray distance in world
+ * units), GL depth test LESS against an internal z-buffer initialised from depth_dev; asynchronous on stream.
+ * Where a fragment wins, rgba8_dev receives its colour (alpha included) and depth_dev its ray distance
+ * length(camera-space position), ready for vr_render_composite.  depth_dev must be >= 0 (1e9 = empty). */
+int vr_draw_meshes(const vr_camera* cam, const vr_mesh_desc* meshes, int n_meshes,
+                   uint8_t* rgba8_dev, float* depth_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -59,6 +59,11 @@ class vr_tree_info(C.Structure):
                 ("device_bytes", C.c_int64)]
 
 
+class vr_mesh_desc(C.Structure):
+    _fields_ = [("vert_dev", C.c_void_p), ("faces_dev", C.c_void_p), ("n_verts", C.c_int32), ("n_faces", C.c_int32),
+                ("face_size", C.c_int32), ("unlit", C.c_int32), ("model", C.c_float * 16)]
+
+
 # name -> (restype, argtypes); every symbol include/volrend_b200.h declares
 SYMBOLS = {
     "vr_default_options": (None, [C.POINTER(vr_options)]),
@@ -111,6 +116,8 @@ SYMBOLS = {
     "vr_launch_count": (C.c_ulonglong, []),
     "vr_last_error": (C.c_char_p, []),
     "vr_version": (C.c_char_p, []),
+    "vr_draw_meshes": (C.c_int, [C.POINTER(vr_camera), C.POINTER(vr_mesh_desc), C.c_int, C.c_void_p, C.c_void_p,
+                                 C.c_void_p]),
 }
 
 _lib = None

@@ -9,6 +9,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -21,6 +22,7 @@
 
 #include "volrend_b200.h"
 #include "vr_kernels.h"
+#include "vr_raster.h"
 #include "vr_types.h"
 
 using namespace vrb;
@@ -1112,6 +1114,77 @@ int vr_probe_lumisphere(const vr_tree* t, const float xyz[3], float* out_dev, vo
     probe_kernel<<<1, 32, 0, (cudaStream_t)stream_>>>(t->dev, xyz[0], xyz[1], xyz[2], n_out, out_dev);
     VR_CUDA(cudaGetLastError());
     g_launches += 1;
+    return VR_OK;
+}
+
+// Mesh pass of cuda_renderer.cpp:103-112 without GL (kernels: vr_raster.cu).  The view matrix is
+// w2c = affineInverse(c2w) (camera.cpp:65), folded with each model matrix in double on the host.
+int vr_draw_meshes(const vr_camera* cam, const vr_mesh_desc* meshes, int n_meshes, uint8_t* rgba8_dev,
+                   float* depth_dev, void* stream) {
+    if (!cam) return fail(VR_EINVAL, "null camera");
+    if (cam->width <= 0 || cam->height <= 0) return fail(VR_EINVAL, "zero-size frame %dx%d", cam->width, cam->height);
+    if (cam->width > kRasterMaxSide || cam->height > kRasterMaxSide)
+        return fail(VR_EINVAL, "frame %dx%d exceeds %d pixels per side", cam->width, cam->height, kRasterMaxSide);
+    if (n_meshes < 0) return fail(VR_EINVAL, "negative mesh count %d", n_meshes);
+    if (n_meshes > 0 && !meshes) return fail(VR_EINVAL, "null mesh array");
+    if (!rgba8_dev || !depth_dev) return fail(VR_EINVAL, "mesh drawing needs colour and depth buffers");
+    const float* c = cam->c2w;  // column-major 3x4: R[r][k] = c[3k + r], translation c[9..11]
+    double R[3][3], inv[3][3];
+    for (int r = 0; r < 3; ++r)
+        for (int k = 0; k < 3; ++k) R[r][k] = c[3 * k + r];
+    const double det = R[0][0] * (R[1][1] * R[2][2] - R[1][2] * R[2][1]) + R[0][1] * (R[1][2] * R[2][0] - R[1][0] * R[2][2]) +
+                       R[0][2] * (R[1][0] * R[2][1] - R[1][1] * R[2][0]);
+    if (!(det != 0.0) || !std::isfinite(det)) return fail(VR_EINVAL, "camera rotation is singular");
+    inv[0][0] = (R[1][1] * R[2][2] - R[1][2] * R[2][1]) / det;
+    inv[0][1] = (R[0][2] * R[2][1] - R[0][1] * R[2][2]) / det;
+    inv[0][2] = (R[0][1] * R[1][2] - R[0][2] * R[1][1]) / det;
+    inv[1][0] = (R[1][2] * R[2][0] - R[1][0] * R[2][2]) / det;
+    inv[1][1] = (R[0][0] * R[2][2] - R[0][2] * R[2][0]) / det;
+    inv[1][2] = (R[0][2] * R[1][0] - R[0][0] * R[1][2]) / det;
+    inv[2][0] = (R[1][0] * R[2][1] - R[1][1] * R[2][0]) / det;
+    inv[2][1] = (R[0][1] * R[2][0] - R[0][0] * R[2][1]) / det;
+    inv[2][2] = (R[0][0] * R[1][1] - R[0][1] * R[1][0]) / det;
+    double V[3][4];  // w2c rows
+    for (int r = 0; r < 3; ++r) {
+        for (int k = 0; k < 3; ++k) V[r][k] = inv[r][k];
+        V[r][3] = -((inv[r][0] * c[9] + inv[r][1] * c[10]) + inv[r][2] * c[11]);
+    }
+    std::vector<RasterMesh> rm;
+    long long total = 0, large_cap = 0;
+    for (int i = 0; i < n_meshes; ++i) {
+        const vr_mesh_desc& d = meshes[i];
+        if (d.face_size < 1 || d.face_size > 3)
+            return fail(VR_EINVAL, "mesh %d: face_size %d (1 = points, 2 = lines, 3 = triangles)", i, d.face_size);
+        if (d.n_verts < 0 || d.n_faces < 0)
+            return fail(VR_EINVAL, "mesh %d: negative count (n_verts %d, n_faces %d)", i, d.n_verts, d.n_faces);
+        if (!d.vert_dev && d.n_verts > 0) return fail(VR_EINVAL, "mesh %d: null vert_dev with %d vertices", i, d.n_verts);
+        const long long np = d.faces_dev ? d.n_faces : d.n_verts / d.face_size;
+        if (np == 0) continue;
+        RasterMesh m{};
+        m.vert = d.vert_dev; m.faces = d.faces_dev;
+        m.n_verts = d.n_verts; m.face_size = d.face_size; m.unlit = d.unlit != 0;
+        const float* M = d.model;  // column-major 4x4: M[r][k] = model[4k + r]
+        for (int k = 0; k < 4; ++k)
+            for (int r = 0; r < 3; ++r)
+                m.mv[3 * k + r] = (float)(((V[r][0] * M[4 * k] + V[r][1] * M[4 * k + 1]) + V[r][2] * M[4 * k + 2]) +
+                                          V[r][3] * M[4 * k + 3]);
+        for (int k = 0; k < 3; ++k)
+            for (int r = 0; r < 3; ++r) m.m3[3 * k + r] = M[4 * k + r];
+        m.base = total; m.n_prims = np;
+        total += np;
+        large_cap += np * (d.face_size == 3 ? 6 : 1);
+        if (total >= kRasterMaxPrims) return fail(VR_EINVAL, "more than %lld primitives in one call", kRasterMaxPrims - 1);
+        rm.push_back(m);
+    }
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
+    if (total == 0) return VR_OK;
+    RasterFrame f{};
+    f.W = cam->width; f.H = cam->height; f.fx = cam->fx; f.fy = cam->fy;
+    f.cx = 0.5f * cam->width; f.cy = 0.5f * cam->height;
+    f.cam_pos[0] = c[9]; f.cam_pos[1] = c[10]; f.cam_pos[2] = c[11];
+    VR_CUDA(raster_draw(f, rm.data(), (int)rm.size(), total, large_cap, rgba8_dev, depth_dev, (cudaStream_t)stream));
+    g_launches += kRasterLaunches;
     return VR_OK;
 }
 

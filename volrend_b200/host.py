@@ -506,12 +506,13 @@ def render_frames_png(tree: N3Tree, cams, options: RenderOptions, paths, n_threa
 
 # ---------------------------------------------------------------------------- VolumeRenderer
 class VolumeRenderer:
-    """GL-free offscreen ``VolumeRenderer`` (renderer.hpp:11-42)."""
+    """GL-free ``VolumeRenderer`` (renderer.hpp:11-42).  ``meshes`` is a list of :class:`volrend_b200.Mesh`;
+    visible ones are rasterized by CUDA and the volume is composited over them."""
 
     def __init__(self):
         self.camera = Camera()
         self.options = RenderOptions()
-        self.meshes = []            # kept for API compatibility; GL meshes are out of scope
+        self.meshes = []            # volrend_b200.mesh.Mesh, drawn in order by render()
         self._tree = None
         self._image = None
         self._depth = None
@@ -534,13 +535,35 @@ class VolumeRenderer:
             self._image = torch.zeros((height, width, 4), dtype=torch.uint8, device="cuda")
         else:
             self._image = None
+        self._depth = None          # ray-distance buffer of the mesh pass, allocated on first use
 
     def render(self):
-        """cuda_renderer.cpp:83-126 without the GL mesh pass: offscreen march into the
-        renderer-owned RGBA8 buffer, which is returned."""
+        """cuda_renderer.cpp:83-126 into the renderer-owned RGBA8 buffer, which is returned.
+
+        With at least one visible mesh this follows the reference's three steps: clear colour to the
+        background as GL does (round(bg * 255), alpha 255) and the ray-distance buffer to 1e9, draw the
+        meshes (:func:`volrend_b200.mesh.draw_meshes`), then composite the volume over them
+        (``launch_renderer(..., offscreen=False)``).  Without one it keeps the offscreen march, whose
+        background is ``background_brightness`` in float rather than the 8-bit cleared colour, so a
+        renderer without meshes renders exactly as it always has."""
         if self._image is None:
             raise RuntimeError("VolumeRenderer needs a CUDA device (no CPU fallback)")
         self.camera._update()
+        visible = [m for m in self.meshes if m.visible]
+        if visible:
+            import torch
+            from .mesh import draw_meshes
+            h, w = self._image.shape[:2]
+            if self._depth is None or tuple(self._depth.shape) != (h, w):
+                self._depth = torch.empty((h, w), dtype=torch.float32, device=self._image.device)
+            bg = round(min(max(float(self.options.background_brightness), 0.0), 1.0) * 255)
+            self._image[..., :3] = bg
+            self._image[..., 3] = 255
+            self._depth.fill_(1e9)
+            draw_meshes(self.camera, visible, self._image, self._depth)
+            if self._tree is not None and self._tree.is_cuda_loaded():
+                launch_renderer(self._tree, self.camera, self.options, self._image, self._depth, None, False)
+            return self._image
         if self._tree is None or not self._tree.is_cuda_loaded():
             bg = int(self.options.background_brightness * 255)
             self._image[..., :3] = bg

@@ -1,0 +1,204 @@
+"""Meshes drawn into the volume render (``include/volrend/mesh.hpp``, ``src/mesh.cpp``), GL-free.
+
+A :class:`Mesh` holds the same fields as the reference's ``volrend::Mesh``; :func:`draw_meshes` rasterizes a
+list of them with the CUDA rasterizer behind ``vr_draw_meshes`` (``volrend_b200/csrc/vr_raster.cu``) into an
+RGBA8 image and a float32 ray-distance buffer, which ``launch_renderer(..., offscreen=False)`` then composites
+the volume into (``VolumeRenderer.render`` does both when it has visible meshes).
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+
+import numpy as np
+
+from . import _capi
+from ._capi import check, lib
+
+VERT_SZ = 9                                   # position, colour, normal (mesh.cpp:26)
+DEFAULT_COLOR = (1.0, 0.5, 0.2)               # mesh.hpp:53,57
+GREY = (0.5, 0.5, 0.5)                        # mesh.hpp:69-78
+
+
+def model_matrix(rotation, translation, scale) -> np.ndarray:
+    """Mesh::draw's model transform (mesh.cpp:368-381): axis-angle rotation (identity below a 1e-3 angle),
+    then uniform scale, then translation.  Returns the 4x4 matrix (float32, row-major indexing M[row, col])."""
+    r = np.asarray(rotation, np.float64).reshape(3)
+    norm = float(np.sqrt(r @ r))
+    m = np.eye(4)
+    if norm >= 1e-3:
+        x, y, z = r / norm
+        s, c = math.sin(norm / 2), math.cos(norm / 2)     # glm::angleAxis -> quaternion (w, x, y, z)
+        qw, qx, qy, qz = c, x * s, y * s, z * s
+        m[:3, :3] = [[1 - 2 * (qy * qy + qz * qz), 2 * (qx * qy - qw * qz), 2 * (qx * qz + qw * qy)],
+                     [2 * (qx * qy + qw * qz), 1 - 2 * (qx * qx + qz * qz), 2 * (qy * qz - qw * qx)],
+                     [2 * (qx * qz - qw * qy), 2 * (qy * qz + qw * qx), 1 - 2 * (qx * qx + qy * qy)]]
+    m[:3, :3] *= float(scale)
+    m[:3, 3] = np.asarray(translation, np.float64).reshape(3)
+    return m.astype(np.float32)
+
+
+class Mesh:
+    """``volrend::Mesh`` (mesh.hpp:9-92): ``vert`` (n_verts * 9 floats), ``faces`` (uint32, empty = consecutive
+    vertices), ``rotation`` (axis-angle), ``translation``, ``scale``, ``face_size`` (3 triangles, 2 lines,
+    1 points), ``visible``, ``unlit``, ``name``.  :meth:`update` uploads vert/faces to the device."""
+
+    def __init__(self, n_verts: int = 0, n_faces: int = 0, face_size: int = 3, unlit: bool = False):
+        self.vert = np.zeros(n_verts * VERT_SZ, np.float32)
+        self.faces = np.zeros(n_faces * face_size, np.uint32)
+        self.rotation = np.zeros(3, np.float32)
+        self.translation = np.zeros(3, np.float32)
+        self.scale = 1.0
+        self.face_size = face_size
+        self.visible = True
+        self.unlit = unlit
+        self.name = "Mesh"
+        self._vert_dev = None
+        self._faces_dev = None
+
+    def update(self) -> None:
+        """Mesh::update (mesh.cpp:339-362): copy the current vert/faces to device memory."""
+        import torch
+        vert = np.ascontiguousarray(self.vert, np.float32).reshape(-1)
+        faces = np.ascontiguousarray(self.faces, np.uint32).reshape(-1)
+        if vert.size % VERT_SZ:
+            raise ValueError(f"Mesh {self.name!r}: vert has {vert.size} floats, not a multiple of {VERT_SZ}")
+        self._vert_dev = torch.from_numpy(vert.copy()).cuda()
+        self._faces_dev = torch.from_numpy(faces.view(np.int32).copy()).cuda() if faces.size else None
+
+    @property
+    def n_verts(self) -> int:
+        return int(np.asarray(self.vert).size // VERT_SZ)
+
+    def model_matrix(self) -> np.ndarray:
+        return model_matrix(self.rotation, self.translation, self.scale)
+
+    def auto_faces(self) -> None:
+        """mesh.cpp:628-631."""
+        self.faces = np.arange(self.n_verts, dtype=np.uint32)
+
+    def _as_c(self) -> _capi.vr_mesh_desc:
+        if self._vert_dev is None:
+            self.update()
+        d = _capi.vr_mesh_desc()
+        n = int(self._vert_dev.numel()) // VERT_SZ
+        d.vert_dev = self._vert_dev.data_ptr() if n else None
+        d.faces_dev = self._faces_dev.data_ptr() if self._faces_dev is not None else None
+        d.n_verts = n
+        d.n_faces = int(self._faces_dev.numel()) // self.face_size if self._faces_dev is not None else 0
+        d.face_size, d.unlit = int(self.face_size), int(bool(self.unlit))
+        col_major = self.model_matrix().T.reshape(16)
+        for i in range(16):
+            d.model[i] = float(col_major[i])
+        return d
+
+    # ---- presets (mesh.cpp:399-626)
+    @staticmethod
+    def Cube(color=DEFAULT_COLOR) -> "Mesh":
+        """Unit cube centred at 0: 36 vertices, 12 triangles, flat normals (mesh.cpp:399-449)."""
+        m = Mesh(36, 0, 3)
+        # faces in the order -z, +z, -y, +y, -x, +x; each is two triangles with corners (a, b) in units of 0.5,
+        # where (a, b) is (x, y) on the z faces, (x, z) on the y faces and (z, y) on the x faces
+        corners = [(-1, -1), (1, 1), (1, -1), (1, 1), (-1, -1), (-1, 1)]
+        v = []
+        for axis, side in [(2, -1), (2, 1), (1, -1), (1, 1), (0, -1), (0, 1)]:
+            normal = [0.0, 0.0, 0.0]
+            normal[axis] = float(side)
+            for a, b in corners:
+                p = [0.0, 0.0, 0.0]
+                p[axis] = 0.5 * side
+                if axis == 2:
+                    p[0], p[1] = 0.5 * a, 0.5 * b
+                elif axis == 1:
+                    p[0], p[2] = 0.5 * a, 0.5 * b
+                else:
+                    p[1], p[2] = 0.5 * b, 0.5 * a
+                v.extend(p + list(color) + normal)
+        m.vert = np.asarray(v, np.float32)
+        m.name = "Cube"
+        return m
+
+    @staticmethod
+    def Sphere(rings: int = 15, sectors: int = 30, color=DEFAULT_COLOR) -> "Mesh":
+        """UV sphere of radius 1: rings*sectors vertices, (rings-1)*sectors*2 triangles (mesh.cpp:451-491)."""
+        m = Mesh(rings * sectors, (rings - 1) * sectors * 2, 3)
+        R = float(np.float32(math.pi / float(np.float32(rings - 1))))
+        S = float(np.float32(2 * math.pi / float(np.float32(sectors))))
+        v = np.zeros((rings, sectors, VERT_SZ), np.float64)
+        for r in range(rings):
+            rR = float(np.float32(r * R))
+            for s in range(sectors):
+                sS = float(np.float32(s * S))
+                z = math.sin(-0.5 * math.pi + rR)
+                x = math.cos(sS) * math.sin(rR)
+                y = math.sin(sS) * math.sin(rR)
+                v[r, s] = (x, y, z, *color, x, y, z)
+        m.vert = v.astype(np.float32).reshape(-1)
+        f = []
+        for r in range(rings - 1):
+            nr = r + 1
+            for s in range(sectors):
+                ns = (s + 1) % sectors
+                f += [r * sectors + ns, r * sectors + s, nr * sectors + s,
+                      nr * sectors + s, nr * sectors + ns, r * sectors + ns]
+        m.faces = np.asarray(f, np.uint32)
+        m.name = "Sphere"
+        return m
+
+    @staticmethod
+    def Line(a, b, color=GREY) -> "Mesh":
+        """One unlit segment a -> b (mesh.cpp:556-568)."""
+        m = Mesh(2, 1, 2)
+        m.vert = np.asarray([*a, *color, 0, 0, 1, *b, *color, 0, 0, 1], np.float32)
+        m.faces = np.asarray([0, 1], np.uint32)
+        m.name = "Line"
+        m.unlit = True
+        return m
+
+    @staticmethod
+    def Lines(points, color=GREY) -> "Mesh":
+        """Polyline through N points (N*3 floats): N-1 unlit segments i -> i+1 (mesh.cpp:570-600)."""
+        p = np.asarray(points, np.float32).reshape(-1)
+        if p.size % 3:
+            print("Lines: Number of elements in points must be divisible by 3")
+        n = p.size // 3
+        m = Mesh(n, max(n - 1, 0), 2)
+        v = m.vert.reshape(n, VERT_SZ)
+        v[:, :3] = p[:3 * n].reshape(n, 3)
+        v[:, 3:6] = color
+        v[:, 6:9] = (0, 0, 1)
+        m.faces = np.stack([np.arange(n - 1), np.arange(1, n)], 1).astype(np.uint32).reshape(-1) if n > 1 else \
+            np.zeros(0, np.uint32)
+        m.name = "Lines"
+        m.unlit = True
+        return m
+
+    @staticmethod
+    def Points(points, color=GREY) -> "Mesh":
+        """Point cloud of N points (N*3 floats), unlit, no faces (mesh.cpp:602-626)."""
+        p = np.asarray(points, np.float32).reshape(-1)
+        if p.size % 3:
+            print("Points: Number of elements in points must be divisible by 3")
+        n = p.size // 3
+        m = Mesh(n, 0, 1)
+        v = m.vert.reshape(n, VERT_SZ)
+        v[:, :3] = p[:3 * n].reshape(n, 3)
+        v[:, 3:6] = color
+        v[:, 6:9] = (0, 0, 1)
+        m.name = "Points"
+        m.unlit = True
+        return m
+
+
+def draw_meshes(cam, meshes, image, depth, stream=None) -> None:
+    """Draws the visible ``meshes`` in order over ``image`` (CUDA uint8 [H,W,4]) and ``depth`` (CUDA float32
+    [H,W], ray distance; GL depth test LESS against it).  Covered pixels receive the mesh colour and the
+    fragment's ray distance.  Meshes never uploaded are uploaded first (:meth:`Mesh.update`)."""
+    from .host import _stream_ptr
+    vis = [m for m in meshes if m.visible]
+    arr = (_capi.vr_mesh_desc * max(len(vis), 1))()
+    for i, m in enumerate(vis):
+        arr[i] = m._as_c()
+    c = cam._as_c()
+    check(lib().vr_draw_meshes(C.byref(c), arr, len(vis), image.data_ptr() if image is not None else None,
+                               depth.data_ptr() if depth is not None else None, _stream_ptr(stream)))
