@@ -257,6 +257,18 @@ typedef struct {
 int vr_draw_meshes(const vr_camera* cam, const vr_mesh_desc* meshes, int n_meshes,
                    uint8_t* rgba8_dev, float* depth_dev, void* stream);
 
+/* ---- octree grid (volrend_b200/csrc/vr_wire.cu) -----------------------------------------------------------
+ * N3Tree::gen_wireframe (src/n3tree.cpp:365-434) generated from the device tree, byte for byte.  Starting at the
+ * root (depth 0), a cell of a node of depth d is emitted when it is a leaf or d >= max_depth, else the walk descends
+ * into it; so max_depth <= 0 gives the root's 8 cells and max_depth >= the tree's depth every leaf.  Each cell
+ * becomes 12 line segments = 24 vertices of 9 floats (position, colour 0,0,0, normal 0,0,1), cells in the
+ * reference's depth-first order, ready for a vr_mesh_desc with face_size 2.  vert_dev NULL: only *n_verts_out is
+ * written.  Otherwise max_verts is the buffer's capacity in vertices (VR_EINVAL, nothing written, if the wireframe
+ * needs more).  The first call on a tree counts its cells per level and synchronises `stream`; later calls are
+ * stream-ordered and take their scratch memory from the stream-ordered allocator. */
+int vr_tree_wireframe(const vr_tree* tree, int max_depth, float* vert_dev, int64_t max_verts,
+                      int64_t* n_verts_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,6 +7,8 @@ built from the reference sources by oracle/Makefile.ref).  Needs a GPU.
       ref_u8   bytes written by volrend::launch_renderer (src/cuda/volrend.cu:166-172)
   python tools/make_golden.py --frames OUT       tests/golden/ref/<frame>.npz, the reference frames the GPU tests
                                                  compare with (golden_cases.REF_FRAMES)
+  python tools/make_golden.py --wire OUT         tests/golden/ref/wire_*.npz, N3Tree::gen_wireframe of the trees and
+                                                 cuts of tests/wire_cases.py
 
 OUT receives the files; copy them to tests/golden/ (or tests/golden/ref/) and commit them.
 """
@@ -22,6 +24,8 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from golden_cases import (CASES, REF_FRAMES, build_case, composite_inputs, ref_frame_record,  # noqa: E402
                           ref_frame_tree, ref_frame_view)
 from oracle import ref_binding as rb  # noqa: E402
+from oracle import ref_wire  # noqa: E402
+from wire_cases import WIRE_DEPTHS, golden_name, record, wire_tree  # noqa: E402
 from volrend_b200 import synth  # noqa: E402
 
 
@@ -83,18 +87,35 @@ def reference_frames(out_dir, only, tmpdir):
         print(name, f"{W}x{H}", "alpha mean %.3f" % f[..., 3].mean(), "rgb mean %.3f" % f[..., :3].mean(), flush=True)
 
 
+def wireframes(out_dir, only, tmpdir):
+    for name, depths in WIRE_DEPTHS.items():
+        if only and name not in only:
+            continue
+        path = os.path.join(tmpdir, name + ".npz")
+        wire_tree(name).save_npz(path)
+        rt = rb.RefTree(path)
+        for d in depths:
+            v = ref_wire.wireframe(rt, d)
+            np.savez_compressed(os.path.join(out_dir, golden_name(name, d) + ".npz"), **record(name, d, v))
+            print(name, "max_depth", d, "cells", v.size // 216, flush=True)
+        rt.close()
+        os.remove(path)
+
+
 def main():
     args = sys.argv[1:]
     frames = "--frames" in args
-    args = [a for a in args if a != "--frames"]
+    wire = "--wire" in args
+    args = [a for a in args if a not in ("--frames", "--wire")]
     if not args:
         raise SystemExit(__doc__)
-    if not rb.available():
-        raise SystemExit(f"{rb.LIB_PATH} is missing: build it with `make ref` where the reference sources are")
+    if not rb.available() or (wire and not ref_wire.available()):
+        lib_path = ref_wire.LIB_PATH if wire else rb.LIB_PATH
+        raise SystemExit(f"{lib_path} is missing: build it with `make ref` where the reference sources are")
     out_dir, only = args[0], args[1:]
     os.makedirs(out_dir, exist_ok=True)
     with tempfile.TemporaryDirectory() as tmpdir:
-        (reference_frames if frames else golden_cases)(out_dir, only, tmpdir)
+        (wireframes if wire else reference_frames if frames else golden_cases)(out_dir, only, tmpdir)
 
 
 if __name__ == "__main__":

@@ -24,6 +24,7 @@
 #include "vr_kernels.h"
 #include "vr_raster.h"
 #include "vr_types.h"
+#include "vr_wire.h"
 
 using namespace vrb;
 
@@ -104,6 +105,10 @@ struct vr_tree {
     vr_tree_info info{};
     int data_dim = 0;
     size_t l2_window_bytes = 0;  // table window kept in persisting L2 (VR_L2_PERSIST=1)
+    // grid wireframe (vr_tree_wireframe): cells per level, counted on the first call
+    std::mutex wire_mu;
+    bool wire_ready = false;
+    WireLevels wire_levels{};
 };
 
 // ------------------------------------------------------------------------------------ upload
@@ -1185,6 +1190,44 @@ int vr_draw_meshes(const vr_camera* cam, const vr_mesh_desc* meshes, int n_meshe
     f.cam_pos[0] = c[9]; f.cam_pos[1] = c[10]; f.cam_pos[2] = c[11];
     VR_CUDA(raster_draw(f, rm.data(), (int)rm.size(), total, large_cap, rgba8_dev, depth_dev, (cudaStream_t)stream));
     g_launches += kRasterLaunches;
+    return VR_OK;
+}
+
+// N3Tree::gen_wireframe (n3tree.cpp:365-434) from the device tables (kernels: vr_wire.cu).
+int vr_tree_wireframe(const vr_tree* t, int max_depth, float* vert_dev, int64_t max_verts, int64_t* n_verts_out,
+                      void* stream_) {
+    if (!t || !n_verts_out) return fail(VR_EINVAL, "null argument");
+    int ndev = 0, dev = -1;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cudaGetDevice(&dev) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
+    }
+    if (dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    vr_tree* mt = const_cast<vr_tree*>(t);
+    WireTree w{};
+    w.wide = t->wide; w.n_tables = t->n_tables; w.wide_p = t->dev.wide_p; w.max_level = t->dev.max_depth;
+    for (int i = 0; i < 3; ++i) { w.offset[i] = t->dev.offset[i]; w.scale[i] = t->dev.scale[i]; }
+    int launches = 0;
+    {
+        std::lock_guard<std::mutex> lk(mt->wire_mu);
+        if (!mt->wire_ready) {
+            const cudaError_t e = wire_levels(w, mt->wire_levels, stream, &launches);
+            g_launches += launches;
+            if (e != cudaSuccess)
+                return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "wireframe cell count: %s", cudaGetErrorString(e));
+            mt->wire_ready = true;
+        }
+    }
+    const long long n = 24 * wire_cells(w, t->wire_levels, max_depth);
+    *n_verts_out = n;
+    if (!vert_dev) return VR_OK;
+    if (max_verts < n) return fail(VR_EINVAL, "the wireframe at max_depth %d has %lld vertices, the buffer holds %lld", max_depth, n, (long long)max_verts);
+    launches = 0;
+    const cudaError_t e = wire_fill(w, t->wire_levels, max_depth, vert_dev, stream, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess)
+        return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "wireframe: %s", cudaGetErrorString(e));
     return VR_OK;
 }
 

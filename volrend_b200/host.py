@@ -275,6 +275,30 @@ class N3Tree:
             self._handle = None
         self._cuda_loaded = False
 
+    # -- grid wireframe (vr_tree_wireframe)
+    def wireframe_vertex_count(self, max_depth: int = 100000) -> int:
+        """Vertices of :meth:`gen_wireframe` ``(max_depth)`` (24 per emitted cell), without generating them."""
+        if not self.is_cuda_loaded():
+            raise RuntimeError("N3Tree is not loaded on the device")
+        n = C.c_int64()
+        check(lib().vr_tree_wireframe(self._handle, int(max_depth), None, 0, C.byref(n), _stream_ptr(None)))
+        return int(n.value)
+
+    def wireframe_device(self, max_depth: int = 100000, stream=None):
+        """:meth:`gen_wireframe` into a new CUDA float32 tensor (flat, 9 floats per vertex), stream-ordered."""
+        import torch
+        n = self.wireframe_vertex_count(max_depth)
+        out = torch.empty(n * 9, dtype=torch.float32, device="cuda")
+        got = C.c_int64()
+        check(lib().vr_tree_wireframe(self._handle, int(max_depth), out.data_ptr(), n, C.byref(got), _stream_ptr(stream)))
+        return out
+
+    def gen_wireframe(self, max_depth: int = 100000) -> np.ndarray:
+        """N3Tree::gen_wireframe (n3tree.cpp:365-434), byte for byte: the octree cut at ``max_depth`` as line
+        segments, 12 per cell = 24 vertices of 9 float32 (position, colour 0, normal 0,0,1).  Generated on the GPU
+        from the device tree and copied to the host."""
+        return self.wireframe_device(max_depth).cpu().numpy()
+
     def info(self) -> dict:
         inf = _capi.vr_tree_info()
         check(lib().vr_tree_get_info(self._handle, C.byref(inf)))
@@ -505,9 +529,13 @@ def render_frames_png(tree: N3Tree, cams, options: RenderOptions, paths, n_threa
 
 
 # ---------------------------------------------------------------------------- VolumeRenderer
+VR_MESH_MAX_VERTS = 2 ** 31 - 1    # vr_mesh_desc.n_verts is int32
+
+
 class VolumeRenderer:
     """GL-free ``VolumeRenderer`` (renderer.hpp:11-42).  ``meshes`` is a list of :class:`volrend_b200.Mesh`;
-    visible ones are rasterized by CUDA and the volume is composited over them."""
+    visible ones are rasterized by CUDA and the volume is composited over them.  ``options.show_grid`` draws the
+    octree cut at ``options.grid_max_depth`` (:meth:`N3Tree.gen_wireframe`) after them, as the reference does."""
 
     def __init__(self):
         self.camera = Camera()
@@ -516,6 +544,8 @@ class VolumeRenderer:
         self._tree = None
         self._image = None
         self._depth = None
+        self._wire = None           # grid mesh (cuda_renderer.cpp wire_) and the depth it was made for
+        self._wire_depth = None     # (last_wire_depth_)
         self.resize(self.camera.width, self.camera.height)
 
     def get_backend(self) -> str:
@@ -524,9 +554,27 @@ class VolumeRenderer:
     def set(self, tree: N3Tree) -> None:
         self._tree = tree           # cuda_renderer.cpp:171-180
         self.options.basis_minmax = [0, max(tree.data_format.basis_dim - 1, 0)]
+        self._wire = self._wire_depth = None
 
     def clear(self) -> None:
         self._tree = None
+        self._wire = self._wire_depth = None
+
+    def _grid_mesh(self):
+        """The grid mesh to draw, or None (cuda_renderer.cpp maybe_gen_wire): regenerated on the device when
+        ``grid_max_depth`` changed since the last one.  Without a loaded tree there is no grid."""
+        if not self.options.show_grid or self._tree is None or not self._tree.is_cuda_loaded():
+            return None
+        depth = int(self.options.grid_max_depth)
+        if self._wire is None or self._wire_depth != depth:
+            from .mesh import Mesh
+            n = self._tree.wireframe_vertex_count(depth)
+            if n > VR_MESH_MAX_VERTS:
+                raise ValueError(f"grid at depth {depth} has {n} vertices; a mesh holds at most {VR_MESH_MAX_VERTS}")
+            self._wire = Mesh._on_device(self._tree.wireframe_device(depth), face_size=2, unlit=True)
+            self._wire.name = "Grid"
+            self._wire_depth = depth
+        return self._wire
 
     def resize(self, width: int, height: int) -> None:
         import torch
@@ -540,16 +588,20 @@ class VolumeRenderer:
     def render(self):
         """cuda_renderer.cpp:83-126 into the renderer-owned RGBA8 buffer, which is returned.
 
-        With at least one visible mesh this follows the reference's three steps: clear colour to the
-        background as GL does (round(bg * 255), alpha 255) and the ray-distance buffer to 1e9, draw the
-        meshes (:func:`volrend_b200.mesh.draw_meshes`), then composite the volume over them
-        (``launch_renderer(..., offscreen=False)``).  Without one it keeps the offscreen march, whose
-        background is ``background_brightness`` in float rather than the 8-bit cleared colour, so a
+        With at least one visible mesh, or the grid (``show_grid`` with a loaded tree), this follows the
+        reference's three steps: clear colour to the background as GL does (round(bg * 255), alpha 255) and the
+        ray-distance buffer to 1e9, draw the meshes and then the grid in one call
+        (:func:`volrend_b200.mesh.draw_meshes`; a mesh wins exact depth ties with the grid), then composite the
+        volume over them (``launch_renderer(..., offscreen=False)``).  Without either it keeps the offscreen
+        march, whose background is ``background_brightness`` in float rather than the 8-bit cleared colour, so a
         renderer without meshes renders exactly as it always has."""
         if self._image is None:
             raise RuntimeError("VolumeRenderer needs a CUDA device (no CPU fallback)")
         self.camera._update()
         visible = [m for m in self.meshes if m.visible]
+        wire = self._grid_mesh()
+        if wire is not None:
+            visible.append(wire)
         if visible:
             import torch
             from .mesh import draw_meshes

@@ -66,6 +66,14 @@ class Mesh:
         self._vert_dev = torch.from_numpy(vert.copy()).cuda()
         self._faces_dev = torch.from_numpy(faces.view(np.int32).copy()).cuda() if faces.size else None
 
+    @classmethod
+    def _on_device(cls, vert_dev, face_size: int, unlit: bool) -> "Mesh":
+        """A mesh drawn straight from a CUDA float32 tensor of vertices it does not own (no faces, identity model);
+        its host ``vert`` stays empty and :meth:`update` is never needed."""
+        m = cls(0, 0, face_size, unlit)
+        m._vert_dev = vert_dev
+        return m
+
     @property
     def n_verts(self) -> int:
         return int(np.asarray(self.vert).size // VERT_SZ)
