@@ -123,7 +123,10 @@ static void trace_one(const orc_tree* tree, const orc_camera* cam, const orc_opt
 }
 
 /* ---- cost model (warp instructions) */
-static double C_SETUP = 330, C_OUT = 25, C_BODY = 105, C_FETCH = 20, C_SHADE = 190;   /* body/fetch: SASS of the r2 queue kernel */
+/* C_BODY / C_FETCH / C_SHADE: SASS of the batch kernel march_persistent_kernel<16, .., 193> as tools/sass_blocks.py
+   counts it (body 77, fetch 19, shade 202 before the funnel-shift table index; 72 / 14 / 199 after).  C_SETUP is
+   an estimate, not a SASS count.  Each constant can be overridden from the environment (C_BODY=77 ...). */
+static double C_SETUP = 330, C_OUT = 25, C_BODY = 72, C_FETCH = 14, C_SHADE = 199;
 static double C_ENQ = 55, C_DRAIN = 250, C_ACC = 10, C_VOTE = 4, C_REFILL = 90, C_BATCH_EXTRA = 40, C_TILE = 30;
 
 typedef struct { double instr, body_iters, body_lanes, shade_iters, shade_lanes, fetch_iters, fetch_lanes; } stats_t;
@@ -342,6 +345,13 @@ int main(int argc, char** argv) {
         const int lv = getenv("LEVELS") ? atoi(getenv("LEVELS")) : 2, g0 = getenv("PHASE") ? atoi(getenv("PHASE")) : lv;
         for (int k = 0; k < 32; ++k) g_b[k] = g0 + k * lv;
         printf("tables: %d levels per step, root table resolves %d\n", lv, g0);
+    }
+    {
+        struct { const char* name; double* v; } cs[] = {{"C_SETUP", &C_SETUP}, {"C_BODY", &C_BODY}, {"C_FETCH", &C_FETCH},
+                                                        {"C_SHADE", &C_SHADE}};
+        for (int k = 0; k < 4; ++k)
+            if (getenv(cs[k].name)) *cs[k].v = atof(getenv(cs[k].name));
+        printf("cost model: C_SETUP %g, C_BODY %g, C_FETCH %g, C_SHADE %g\n", C_SETUP, C_BODY, C_FETCH, C_SHADE);
     }
     pthread_once(&g_h2f_once, init_h2f);
     orc_tree tree;
