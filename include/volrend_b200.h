@@ -20,6 +20,8 @@
  *   vr_render_frames_host              main_headless.cpp:208-223 with `-o`: renders and
  *                                      copies every frame to host memory (:216-219)
  *   vr_probe_lumisphere                retrieve_cursor_lumisphere_kernel (volrend.cu:175-191)
+ *   vr_draw_probe                      the enable_probe disc of render_kernel (volrend.cu:100-134),
+ *                                      drawn over frames the calls above have written
  *   vr_last_error                      replaces the abort-on-error cuda_assert
  *                                      (src/cuda/common.cu:8-21) -- the C-ABI never aborts;
  *                                      the C++ shim (volrend_b200/csrc/shim) restores it.
@@ -176,6 +178,22 @@ int vr_render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views
 /* Copies the colour coefficients of the leaf containing world point xyz into out_dev as floats
  * (retrieve_cursor_lumisphere_kernel): min(data_dim-1, 3*basis_dim) values (3 for RGBA). */
 int vr_probe_lumisphere(const vr_tree* tree, const float xyz_world[3], float* out_dev, void* stream);
+
+/* RenderOptions::enable_probe (volrend.cu:100-134): draws the lumisphere probe disc of the leaf containing world point
+ * probe_xyz over n_views frames that vr_render / vr_render_batch / vr_render_composite / vr_render_surface already
+ * wrote with the same cams, tile and layout (one launch, stream-ordered after them).  disp_size is probe_disp_size:
+ * the disc spans the top-right disp_size x disp_size pixels of the full frame, 5 pixels in from the right and down
+ * from the top edge; of a `tile` only the part inside it is written, at tile-relative positions.  A disc pixel gets
+ * the leaf's colour seen along the direction the disc point faces (the camera rotation applied to the point of the
+ * unit hemisphere behind it), alpha 1: sigmoid of the basis sum for SH/SG/ASG trees, the raw RGB for RGBA trees; the
+ * byte and float outputs hold what the reference's render_kernel stores there.  Pixels outside the disc are left as
+ * they are.  Of `opt` only basis_minmax is read, clamped to the tree's basis (the reference reads past the
+ * coefficients when the range reaches beyond basis_dim - 1).  rgba8_surf != 0 selects the surface form: one view,
+ * tile NULL, rgba8_dev and rgba32f_dev NULL.  disp_size <= 0 draws nothing.  VR_EUNSUPPORTED for the trees
+ * vr_probe_lumisphere refuses. */
+int vr_draw_probe(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
+                  const float probe_xyz[3], int disp_size, const vr_rect* tile,
+                  uint8_t* rgba8_dev, float* rgba32f_dev, unsigned long long rgba8_surf, void* stream);
 
 /* Diagnostics: one full-frame render with the instrumented kernel that also records, per 8x4-pixel
  * work item (row-major tiles of 8x4), {start ns, end ns, SM id, global warp id} into

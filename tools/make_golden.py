@@ -9,6 +9,8 @@ built from the reference sources by oracle/Makefile.ref).  Needs a GPU.
                                                  compare with (golden_cases.REF_FRAMES)
   python tools/make_golden.py --wire OUT         tests/golden/ref/wire_*.npz, N3Tree::gen_wireframe of the trees and
                                                  cuts of tests/wire_cases.py
+  python tools/make_golden.py --probe OUT        tests/golden/ref/probe_*.npz, launch_renderer with enable_probe (and
+                                                 the same frame without it) for the cases of tests/probe_cases.py
 
 OUT receives the files; copy them to tests/golden/ (or tests/golden/ref/) and commit them.
 """
@@ -24,7 +26,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from golden_cases import (CASES, REF_FRAMES, build_case, composite_inputs, ref_frame_record,  # noqa: E402
                           ref_frame_tree, ref_frame_view)
 from oracle import ref_binding as rb  # noqa: E402
+from oracle import probe_oracle  # noqa: E402
 from oracle import ref_wire  # noqa: E402
+from probe_cases import PROBE_CASES, golden_path, probe_case  # noqa: E402
 from wire_cases import WIRE_DEPTHS, golden_name, record, wire_tree  # noqa: E402
 from volrend_b200 import synth  # noqa: E402
 
@@ -102,20 +106,44 @@ def wireframes(out_dir, only, tmpdir):
         os.remove(path)
 
 
+def probe_frames(out_dir, only, tmpdir):
+    for name in PROBE_CASES:
+        if only and name not in only:
+            continue
+        st, pose, optkw, probe, disp, comp = probe_case(name)
+        path = os.path.join(tmpdir, name + ".npz")
+        st.save_npz(path)
+        import probe_cases as pc
+        fx = pc.focal()
+        c12 = synth.c2w_to_colmajor12(pose)
+        rin, din = comp if comp is not None else (None, None)
+        u = probe_oracle.ref_render_u8(path, pc.W, pc.H, fx, fx, c12, probe_oracle.ref_options(probe, disp, **optkw),
+                                       rgba_in=rin, depth_in=din)
+        rt = rb.RefTree(path)
+        u_off = rt.render_u8(pc.W, pc.H, fx, fx, c12, rb.make_options(**optkw), rgba_in=rin, depth_in=din)
+        rt.close()
+        os.remove(path)
+        np.savez_compressed(os.path.join(out_dir, os.path.basename(golden_path(name))), case=np.array(name),
+                            ref_u8=u, ref_u8_off=u_off)
+        print(name, "disc pixels changed", int((u != u_off).any(-1).sum()), flush=True)
+
+
 def main():
     args = sys.argv[1:]
     frames = "--frames" in args
     wire = "--wire" in args
-    args = [a for a in args if a not in ("--frames", "--wire")]
+    probe = "--probe" in args
+    args = [a for a in args if a not in ("--frames", "--wire", "--probe")]
     if not args:
         raise SystemExit(__doc__)
-    if not rb.available() or (wire and not ref_wire.available()):
-        lib_path = ref_wire.LIB_PATH if wire else rb.LIB_PATH
+    if not rb.available() or (wire and not ref_wire.available()) or (probe and not probe_oracle.ref_available()):
+        lib_path = ref_wire.LIB_PATH if wire else probe_oracle.REF_PATH if probe else rb.LIB_PATH
         raise SystemExit(f"{lib_path} is missing: build it with `make ref` where the reference sources are")
     out_dir, only = args[0], args[1:]
     os.makedirs(out_dir, exist_ok=True)
     with tempfile.TemporaryDirectory() as tmpdir:
-        (wireframes if wire else reference_frames if frames else golden_cases)(out_dir, only, tmpdir)
+        run = wireframes if wire else probe_frames if probe else reference_frames if frames else golden_cases
+        run(out_dir, only, tmpdir)
 
 
 if __name__ == "__main__":

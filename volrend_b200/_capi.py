@@ -85,6 +85,8 @@ SYMBOLS = {
     "vr_render_frames_png": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
                                        C.POINTER(C.c_char_p), C.c_int]),
     "vr_probe_lumisphere": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_void_p, C.c_void_p]),
+    "vr_draw_probe": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options), C.POINTER(C.c_float),
+                                C.c_int, C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p]),
     "vr_render_bands": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.POINTER(vr_options), C.c_int, C.c_int, C.c_int,
                                   C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_band_rows": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int]),

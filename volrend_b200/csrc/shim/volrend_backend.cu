@@ -161,13 +161,18 @@ __host__ void launch_renderer(const N3Tree& tree, const Camera& cam, const Rende
         }
         dsurf = surface_for(depth_arr);
     }
-    if (options.enable_probe) {
-        // lumisphere probe overlay (volrend.cu:100-134) is a GUI feature outside the ray path
-        static bool warned = false;
-        if (!warned) { fprintf(stderr, "volrend_b200: enable_probe overlay is not drawn by this backend\n"); warned = true; }
-    }
     const int rc = vr_render_surface(t, &c, &o, (unsigned long long)surf, (unsigned long long)dsurf, (void*)stream);
     if (rc != VR_OK) die("vr_render_surface", rc);
+    if (options.enable_probe) {   // the lumisphere probe disc of volrend.cu:100-134
+        const int prc = vr_draw_probe(t, &c, 1, &o, options.probe, options.probe_disp_size, nullptr, nullptr, nullptr,
+                                      (unsigned long long)surf, (void*)stream);
+        if (prc == VR_EUNSUPPORTED) {
+            static bool warned = false;
+            if (!warned) { fprintf(stderr, "volrend_b200: enable_probe disc not drawn: %s\n", vr_last_error()); warned = true; }
+        } else if (prc != VR_OK) {
+            die("vr_draw_probe", prc);
+        }
+    }
 }
 
 // ---------------------------------------------------------------- VolumeRenderer (GL-free)

@@ -8,6 +8,7 @@
 
 #include <cub/device/device_scan.cuh>
 
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
@@ -22,6 +23,7 @@
 
 #include "volrend_b200.h"
 #include "vr_kernels.h"
+#include "vr_probe.h"
 #include "vr_raster.h"
 #include "vr_types.h"
 #include "vr_wire.h"
@@ -387,22 +389,7 @@ __global__ void queue_init_kernel(unsigned char* slots) {
 
 // retrieve_cursor_lumisphere_kernel (volrend.cu:175-191): descends the wide tables.
 __global__ void probe_kernel(TreeDev tree, float x, float y, float z, int n_out, float* __restrict__ out) {
-    float p[3] = {tree.offset[0] + tree.scale[0] * x, tree.offset[1] + tree.scale[1] * y,
-                  tree.offset[2] + tree.scale[2] * z};
-    uint32_t u[3];
-    for (int i = 0; i < 3; ++i) {
-        p[i] = fmaxf(fminf(p[i], 1.f - 1e-6f), 0.f);
-        u[i] = __float2uint_rz(p[i] * tree.pos_scale);
-    }
-    uint32_t T = 0, eidx = 0;
-    constexpr uint32_t M = (1u << kWideLv) - 1u;
-    for (int j = 0; j < 16; ++j) {
-        const int sh = (24 - kWideLv) - kWideLv * j;
-        eidx = T * (uint32_t)kWideEntries + ((((u[0] >> sh) & M) << (2 * kWideLv)) | (((u[1] >> sh) & M) << kWideLv) | ((u[2] >> sh) & M));
-        const uint32_t w = tree.wide[eidx];
-        if (w & kLeafBit) break;
-        T = w;
-    }
+    const uint32_t eidx = probe_leaf_entry(tree, x, y, z);
     const unsigned short* rec = reinterpret_cast<const unsigned short*>(tree.wrecs + (size_t)eidx * tree.rec_bytes);
     for (int i = threadIdx.x; i < n_out; i += blockDim.x) out[i] = __half2float(__ushort_as_half(rec[i]));
 }
@@ -1118,6 +1105,69 @@ int vr_probe_lumisphere(const vr_tree* t, const float xyz[3], float* out_dev, vo
     const int n_out = t->data_dim - 1 < resident ? t->data_dim - 1 : resident;
     probe_kernel<<<1, 32, 0, (cudaStream_t)stream_>>>(t->dev, xyz[0], xyz[1], xyz[2], n_out, out_dev);
     VR_CUDA(cudaGetLastError());
+    g_launches += 1;
+    return VR_OK;
+}
+
+// The probe disc of render_kernel (volrend.cu:100-134) over frames the march has written (kernel: vr_probe.cu).
+int vr_draw_probe(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, const float probe_xyz[3],
+                  int disp_size, const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev,
+                  unsigned long long rgba8_surf, void* stream_) {
+    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
+    if (!probe_xyz) return fail(VR_EINVAL, "null probe position");
+    if (rgba8_surf) {
+        if (n_views != 1 || tile || rgba8_dev || rgba32f_dev)
+            return fail(VR_EINVAL, "the surface form draws one full frame and no linear or float output");
+    } else if (!rgba8_dev && !rgba32f_dev) {
+        return fail(VR_EINVAL, "no output to draw into");
+    }
+    if (n_views == 0) return VR_OK;
+    vr_rect r;
+    int rc = check_common(t, cams, opt, tile, r);
+    if (rc) return rc;
+    for (int i = 1; i < n_views; ++i)
+        if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
+            return fail(VR_EINVAL, "all views of a batch must share one image size");
+    if (t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim)
+        return fail(VR_EUNSUPPORTED, "probe unavailable for basis_dim %d (only coefficient 0 is resident)", t->dev.basis_dim);
+    if (disp_size <= 0) return VR_OK;   // the reference's candidate pixels then all lie outside the disc
+    // candidate corner, volrend.cu:100-101: y < S + 5 && x >= W - S - 5, in the 32-bit wrapping adds of the SASS
+    const int W = cams[0].width, H = cams[0].height;
+    const int y_end = (int)((uint32_t)disp_size + 5u), x_beg = (int)((uint32_t)W - (uint32_t)disp_size - 5u);
+    const int cx0 = std::max(std::max(x_beg, 0), r.x0), cx1 = std::min(W, r.x0 + r.w);
+    const int cy0 = r.y0, cy1 = std::min(std::min(y_end, H), r.y0 + r.h);
+    if (cx0 >= cx1 || cy0 >= cy1) return VR_OK;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (n_views > kCamRing) {
+        const size_t tile_px = (size_t)r.w * r.h;
+        for (int v0 = 0; v0 < n_views; v0 += kCamRing) {
+            const int nv = n_views - v0 < kCamRing ? n_views - v0 : kCamRing;
+            rc = vr_draw_probe(t, cams + v0, nv, opt, probe_xyz, disp_size, tile, rgba8_dev ? rgba8_dev + 4 * tile_px * v0 : nullptr,
+                               rgba32f_dev ? rgba32f_dev + 4 * tile_px * v0 : nullptr, 0, stream_);
+            if (rc) return rc;
+        }
+        return VR_OK;
+    }
+    ProbeLaunch P{};
+    P.tree = t->dev;
+    for (int i = 0; i < 3; ++i) P.probe[i] = probe_xyz[i];
+    P.disp = disp_size;
+    // the reference sums basis_minmax[0]..[1] and reads past the coefficients when the range leaves the tree's
+    // basis; here it is clamped to the basis, as the march clamps it
+    const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
+    P.bmin = std::max(opt->basis_minmax[0], 0);
+    P.bmax = std::min(opt->basis_minmax[1], nb - 1);
+    fill_cam(P.cam, &cams[0]);
+    P.n_views = n_views;
+    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
+    P.cx0 = cx0; P.cy0 = cy0; P.cw = cx1 - cx0; P.ch = cy1 - cy0;
+    P.rgba8 = rgba8_dev; P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
+    P.surf = (cudaSurfaceObject_t)rgba8_surf;
+    LaunchDev L{};
+    if ((rc = stage_cams(t, cams, n_views, stream, L))) return rc;
+    P.cams = n_views > 1 ? L.cams : nullptr;
+    const cudaError_t e = probe_draw(P, t->dev.kbd, stream);
+    if (e != cudaSuccess) return fail(VR_ECUDA, "probe overlay launch failed: %s", cudaGetErrorString(e));
     g_launches += 1;
     return VR_OK;
 }

@@ -421,6 +421,16 @@ def launch_renderer(tree: N3Tree, cam: Camera, options: RenderOptions, image_arr
             raise ValueError("offscreen=False needs colour and depth inputs")
         check(lib().vr_render_composite(tree._handle, C.byref(c), C.byref(o), _rect(tile), img,
                                         depth_arr.data_ptr(), fo, s))
+    if options.enable_probe:
+        _draw_probe(tree, (c,), 1, options, o, tile, img, fo, s)
+
+
+def _draw_probe(tree: N3Tree, cams, n_views: int, options: RenderOptions, o, tile, img, fo, s) -> None:
+    """The ``enable_probe`` disc (volrend.cu:100-134) over the frames just rendered: one vr_draw_probe launch."""
+    arr = cams if isinstance(cams, C.Array) else (_capi.vr_camera * n_views)(*cams)
+    xyz = (C.c_float * 3)(*[float(v) for v in options.probe])
+    check(lib().vr_draw_probe(tree._handle, arr, n_views, C.byref(o), xyz, int(options.probe_disp_size), _rect(tile),
+                              img, fo, 0, s))
 
 
 def render_bands(tree: N3Tree, cam: Camera, options: RenderOptions, band_h: int, n_parts: int, part: int,
@@ -496,10 +506,13 @@ def render_batch(tree: N3Tree, cams, options: RenderOptions, images, *, float_ou
     """The pose loop of main_headless.cpp:208-223 as one call; ``images``: uint8 [V,H,W,4]."""
     arr = _cams_array(cams)
     o = options._as_c()
-    check(lib().vr_render_batch(tree._handle, arr, len(cams), C.byref(o), _rect(tile),
-                                images.data_ptr() if images is not None else None,
-                                float_out.data_ptr() if float_out is not None else None,
-                                counters.data_ptr() if counters is not None else None, _stream_ptr(stream)))
+    img = images.data_ptr() if images is not None else None
+    fo = float_out.data_ptr() if float_out is not None else None
+    s = _stream_ptr(stream)
+    check(lib().vr_render_batch(tree._handle, arr, len(cams), C.byref(o), _rect(tile), img, fo,
+                                counters.data_ptr() if counters is not None else None, s))
+    if options.enable_probe and len(cams):
+        _draw_probe(tree, arr, len(cams), options, o, tile, img, fo, s)
 
 
 def render_frames_host(tree: N3Tree, cams, options: RenderOptions, host_images) -> None:
@@ -532,10 +545,26 @@ def render_frames_png(tree: N3Tree, cams, options: RenderOptions, paths, n_threa
 VR_MESH_MAX_VERTS = 2 ** 31 - 1    # vr_mesh_desc.n_verts is int32
 
 
+def _probe_cube():
+    """The probe marker of cuda_renderer.cpp:25-38: an unlit black cube whose +-z faces are blue, +-y faces green
+    and +-x faces red, at scale 0.05 and hidden."""
+    from .mesh import VERT_SZ, Mesh
+    m = Mesh.Cube((0.0, 0.0, 0.0))
+    v = m.vert.reshape(36, VERT_SZ)
+    for i in range(3):
+        v[12 * i:12 * (i + 1), 3 + 2 - i] = 1.0
+    m.name = "_probe_cube"
+    m.visible = False
+    m.scale = 0.05
+    m.unlit = True
+    return m
+
+
 class VolumeRenderer:
     """GL-free ``VolumeRenderer`` (renderer.hpp:11-42).  ``meshes`` is a list of :class:`volrend_b200.Mesh`;
-    visible ones are rasterized by CUDA and the volume is composited over them.  ``options.show_grid`` draws the
-    octree cut at ``options.grid_max_depth`` (:meth:`N3Tree.gen_wireframe`) after them, as the reference does."""
+    visible ones are rasterized by CUDA and the volume is composited over them.  ``options.enable_probe`` draws the
+    probe cube at ``options.probe`` after them, and ``options.show_grid`` the octree cut at
+    ``options.grid_max_depth`` (:meth:`N3Tree.gen_wireframe`) after that, as the reference does."""
 
     def __init__(self):
         self.camera = Camera()
@@ -546,6 +575,7 @@ class VolumeRenderer:
         self._depth = None
         self._wire = None           # grid mesh (cuda_renderer.cpp wire_) and the depth it was made for
         self._wire_depth = None     # (last_wire_depth_)
+        self._probe = _probe_cube()  # (probe_)
         self.resize(self.camera.width, self.camera.height)
 
     def get_backend(self) -> str:
@@ -554,6 +584,7 @@ class VolumeRenderer:
     def set(self, tree: N3Tree) -> None:
         self._tree = tree           # cuda_renderer.cpp:171-180
         self.options.basis_minmax = [0, max(tree.data_format.basis_dim - 1, 0)]
+        self._probe.scale = float(np.float32(0.02) / np.float32(tree.scale[0]))
         self._wire = self._wire_depth = None
 
     def clear(self) -> None:
@@ -588,17 +619,22 @@ class VolumeRenderer:
     def render(self):
         """cuda_renderer.cpp:83-126 into the renderer-owned RGBA8 buffer, which is returned.
 
-        With at least one visible mesh, or the grid (``show_grid`` with a loaded tree), this follows the
-        reference's three steps: clear colour to the background as GL does (round(bg * 255), alpha 255) and the
-        ray-distance buffer to 1e9, draw the meshes and then the grid in one call
-        (:func:`volrend_b200.mesh.draw_meshes`; a mesh wins exact depth ties with the grid), then composite the
-        volume over them (``launch_renderer(..., offscreen=False)``).  Without either it keeps the offscreen
-        march, whose background is ``background_brightness`` in float rather than the 8-bit cleared colour, so a
-        renderer without meshes renders exactly as it always has."""
+        With at least one visible mesh, the probe cube (``enable_probe``) or the grid (``show_grid`` with a loaded
+        tree), this follows the reference's three steps: clear colour to the background as GL does
+        (round(bg * 255), alpha 255) and the ray-distance buffer to 1e9, draw the meshes, the probe cube and then
+        the grid in one call (:func:`volrend_b200.mesh.draw_meshes`; an earlier one wins exact depth ties), then
+        composite the volume over them (``launch_renderer(..., offscreen=False)``, which also draws the probe
+        disc).  Without any of them it keeps the offscreen march, whose background is ``background_brightness`` in
+        float rather than the 8-bit cleared colour, so a renderer without meshes renders exactly as it always
+        has."""
         if self._image is None:
             raise RuntimeError("VolumeRenderer needs a CUDA device (no CPU fallback)")
         self.camera._update()
         visible = [m for m in self.meshes if m.visible]
+        self._probe.visible = bool(self.options.enable_probe)      # cuda_renderer.cpp:94-95
+        self._probe.translation = np.asarray(self.options.probe, np.float32).reshape(3).copy()
+        if self._probe.visible:
+            visible.append(self._probe)
         wire = self._grid_mesh()
         if wire is not None:
             visible.append(wire)
