@@ -4,7 +4,7 @@
 #                 oracle/libprobe_oracle.so         the same with the probe disc
 #   make exp      volrend_b200/libvolrend_b200_exp.so  the same library with the measured experiment kernels
 #                                                   (-DVR_EXPERIMENTS; the parity tests check them)
-#   make ref      oracle/_ref/*                     the unmodified reference (+ its gen_wireframe and probe harnesses), built from
+#   make ref      oracle/_ref/*                     the unmodified reference (+ its gen_wireframe, probe and mesh harnesses), built from
 #                                                   $(VOLREND_REF) (only when it exists)
 #   make shim     oracle/_ref/volrend_headless ...  reference CLI linked against OUR backend
 NVCC      ?= nvcc
@@ -42,7 +42,7 @@ $(OBJ)/vr_kernels_%.o: volrend_b200/csrc/vr_kernels_inst.cu volrend_b200/csrc/vr
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -DVR_KBD=$* -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_$*.log || (cat $(OBJ)/ptxas_$*.log; false)
 
-$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h include/volrend_b200.h
+$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -53,6 +53,10 @@ $(OBJ)/vr_raster.o: volrend_b200/csrc/vr_raster.cu volrend_b200/csrc/vr_raster.h
 $(OBJ)/vr_wire.o: volrend_b200/csrc/vr_wire.cu volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_types.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_wire.log || (cat $(OBJ)/ptxas_wire.log; false)
+
+$(OBJ)/vr_normals.o: volrend_b200/csrc/vr_normals.cu volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_raster.h
+	@mkdir -p $(OBJ)
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_normals.log || (cat $(OBJ)/ptxas_normals.log; false)
 
 $(OBJ)/vr_probe.o: volrend_b200/csrc/vr_probe.cu volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_types.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
@@ -66,7 +70,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(CXX) -O3 -std=c++17 -fPIC -Iinclude -c $< -o $@
 
-$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_probe.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
+$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_probe.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
 oracle: oracle/liboracle.so oracle/libprobe_oracle.so
@@ -78,7 +82,8 @@ oracle/libprobe_oracle.so: oracle/probe_oracle.c oracle/march_oracle.c oracle/ma
 ref:
 	@if [ -d "$(VOLREND_REF)/src/cuda" ]; then $(MAKE) -C oracle -f Makefile.ref VOLREND_REF=$(VOLREND_REF) && \
 	   $(MAKE) -C oracle -f Makefile.wire VOLREND_REF=$(VOLREND_REF) && \
-	   $(MAKE) -C oracle -f Makefile.probe VOLREND_REF=$(VOLREND_REF); \
+	   $(MAKE) -C oracle -f Makefile.probe VOLREND_REF=$(VOLREND_REF) && \
+	   $(MAKE) -C oracle -f Makefile.mesh VOLREND_REF=$(VOLREND_REF); \
 	 else echo "reference tree $(VOLREND_REF) not present: using prebuilt oracle/_ref if any"; fi
 
 shim:

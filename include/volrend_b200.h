@@ -287,6 +287,17 @@ int vr_draw_meshes(const vr_camera* cam, const vr_mesh_desc* meshes, int n_meshe
 int vr_tree_wireframe(const vr_tree* tree, int max_depth, float* vert_dev, int64_t max_verts,
                       int64_t* n_verts_out, void* stream);
 
+/* ---- mesh normals (volrend_b200/csrc/vr_normals.cu) ------------------------------------------------------
+ * Mesh estimate_normals (src/mesh.cpp:63-97), byte for byte: overwrites floats 6..8 (the normal) of each 9-float
+ * vertex of vert_dev with the normalised sum of the cross products of its incident triangles, added in face order
+ * from +0.f (vertices without faces get 0,0,0); every other float is left alone.  faces_dev NULL: a triangle soup,
+ * n_verts / 3 faces of consecutive vertex triples (n_faces is ignored).  Otherwise n_faces triangles of 3 indices;
+ * a face with an index >= n_verts contributes nothing.  Asynchronous on stream; scratch comes from the
+ * rasterizer's stream-ordered pool.  VR_EINVAL for negative counts, NULL vert_dev with n_verts > 0, or more than
+ * 2^31-1 vertices or face corners. */
+int vr_mesh_estimate_normals(float* vert_dev, int64_t n_verts, const uint32_t* faces_dev, int64_t n_faces,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif

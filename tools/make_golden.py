@@ -11,6 +11,9 @@ built from the reference sources by oracle/Makefile.ref).  Needs a GPU.
                                                  cuts of tests/wire_cases.py
   python tools/make_golden.py --probe OUT        tests/golden/ref/probe_*.npz, launch_renderer with enable_probe (and
                                                  the same frame without it) for the cases of tests/probe_cases.py
+  python tools/make_golden.py --mesh OUT         tests/golden/ref/mesh_*.npz, Mesh::open_drawlist_mem and
+                                                 Mesh::load_mem_basic_obj of the inputs of tests/mesh_io_cases.py
+                                                 (needs only oracle/_ref/libref_mesh.so, no GPU)
 
 OUT receives the files; copy them to tests/golden/ (or tests/golden/ref/) and commit them.
 """
@@ -128,8 +131,34 @@ def probe_frames(out_dir, only, tmpdir):
         print(name, "disc pixels changed", int((u != u_off).any(-1).sum()), flush=True)
 
 
+def mesh_loads(out_dir, only, tmpdir):
+    import mesh_io_cases as mc
+    from oracle import ref_mesh
+    for name, (data, vis, normals) in mc.drawlist_cases().items():
+        if not only or name in only:
+            rec = mc.record("drawlist", data, ref_mesh.open_drawlist_mem(data, vis), vis, normals)
+            np.savez_compressed(os.path.join(out_dir, "mesh_" + name + ".npz"), **rec)
+            print(name, "meshes", int(rec["n"]), flush=True)
+    for name, (text, normals) in mc.obj_cases().items():
+        if not only or name in only:
+            data = text.encode("latin-1")
+            rec = mc.record("obj", data, [ref_mesh.load_mem_obj(data)], True, normals)
+            np.savez_compressed(os.path.join(out_dir, "mesh_" + name + ".npz"), **rec)
+            print(name, "vertices", rec["m0_vert"].size // 9, flush=True)
+
+
 def main():
     args = sys.argv[1:]
+    if "--mesh" in args:                # CPU only: the reference's Mesh loaders
+        from oracle import ref_mesh
+        args = [a for a in args if a != "--mesh"]
+        if not args:
+            raise SystemExit(__doc__)
+        if not ref_mesh.available():
+            raise SystemExit(f"{ref_mesh.LIB_PATH} is missing: build it with `make ref` where the reference sources are")
+        os.makedirs(args[0], exist_ok=True)
+        mesh_loads(args[0], args[1:], None)
+        return
     frames = "--frames" in args
     wire = "--wire" in args
     probe = "--probe" in args

@@ -121,6 +121,7 @@ SYMBOLS = {
     "vr_draw_meshes": (C.c_int, [C.POINTER(vr_camera), C.POINTER(vr_mesh_desc), C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p]),
     "vr_tree_wireframe": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
+    "vr_mesh_estimate_normals": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
 }
 
 _lib = None

@@ -23,6 +23,7 @@
 
 #include "volrend_b200.h"
 #include "vr_kernels.h"
+#include "vr_normals.h"
 #include "vr_probe.h"
 #include "vr_raster.h"
 #include "vr_types.h"
@@ -1278,6 +1279,29 @@ int vr_tree_wireframe(const vr_tree* t, int max_depth, float* vert_dev, int64_t 
     g_launches += launches;
     if (e != cudaSuccess)
         return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "wireframe: %s", cudaGetErrorString(e));
+    return VR_OK;
+}
+
+
+// estimate_normals (mesh.cpp:63-97) on a device vertex buffer (kernels: vr_normals.cu).
+int vr_mesh_estimate_normals(float* vert_dev, int64_t n_verts, const uint32_t* faces_dev, int64_t n_faces,
+                             void* stream) {
+    if (n_verts < 0 || n_faces < 0)
+        return fail(VR_EINVAL, "negative count (n_verts %lld, n_faces %lld)", (long long)n_verts, (long long)n_faces);
+    if (!vert_dev && n_verts > 0) return fail(VR_EINVAL, "null vert_dev with %lld vertices", (long long)n_verts);
+    if (n_verts > INT32_MAX) return fail(VR_EINVAL, "%lld vertices: at most %d", (long long)n_verts, INT32_MAX);
+    if (faces_dev && n_faces > INT32_MAX / 3)
+        return fail(VR_EINVAL, "%lld faces: at most %d face corners", (long long)n_faces, INT32_MAX);
+    int ndev = 0, dev = -1;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cudaGetDevice(&dev) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
+    }
+    int launches = 0;
+    const cudaError_t e = normals_estimate(vert_dev, n_verts, faces_dev, n_faces, (cudaStream_t)stream, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess)
+        return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "mesh normals: %s", cudaGetErrorString(e));
     return VR_OK;
 }
 

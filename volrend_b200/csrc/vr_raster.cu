@@ -420,6 +420,8 @@ __global__ void __launch_bounds__(128) resolve(const RasterMesh* __restrict__ me
     depth[p] = dist;
 }
 
+}  // namespace
+
 // Scratch comes from a memory pool of the rasterizer's own per device, which keeps what it has reserved (the
 // default pool returns memory at every synchronisation, and re-mapping it cost more than the draw itself).
 // Allocation is stream-ordered, so concurrent calls on different streams never share scratch.
@@ -445,8 +447,6 @@ cudaError_t scratch_pool(cudaMemPool_t* out) {
     *out = pools[dev];
     return cudaSuccess;
 }
-
-}  // namespace
 
 cudaError_t raster_draw(const RasterFrame& f, const RasterMesh* meshes, int n, long long total_prims,
                         long long large_cap, uint8_t* rgba8, float* depth, cudaStream_t st) {

@@ -34,4 +34,8 @@ cudaError_t raster_draw(const RasterFrame& f, const RasterMesh* meshes, int n, l
                         long long large_cap, uint8_t* rgba8, float* depth, cudaStream_t stream);
 constexpr int kRasterLaunches = 4;
 
+// The rasterizer's stream-ordered scratch pool of the current device (it keeps what it has reserved); the normal
+// estimation (vr_normals.cu) allocates from it too.
+cudaError_t scratch_pool(cudaMemPool_t* out);
+
 }  // namespace vrb

@@ -3,11 +3,14 @@
 A :class:`Mesh` holds the same fields as the reference's ``volrend::Mesh``; :func:`draw_meshes` rasterizes a
 list of them with the CUDA rasterizer behind ``vr_draw_meshes`` (``volrend_b200/csrc/vr_raster.cu``) into an
 RGBA8 image and a float32 ray-distance buffer, which ``launch_renderer(..., offscreen=False)`` then composites
-the volume into (``VolumeRenderer.render`` does both when it has visible meshes).
+the volume into (``VolumeRenderer.render`` does both when it has visible meshes).  Meshes also come from drawlist
+``.npz`` files and OBJ files (:meth:`Mesh.open_drawlist`, :meth:`Mesh.load_basic_obj`, in ``mesh_io.py``), whose
+normals :func:`estimate_normals` computes with a CUDA kernel (``volrend_b200/csrc/vr_normals.cu``).
 """
 from __future__ import annotations
 
 import ctypes as C
+import ctypes.util
 import math
 
 import numpy as np
@@ -18,6 +21,33 @@ from ._capi import check, lib
 VERT_SZ = 9                                   # position, colour, normal (mesh.cpp:26)
 DEFAULT_COLOR = (1.0, 0.5, 0.2)               # mesh.hpp:53,57
 GREY = (0.5, 0.5, 0.5)                        # mesh.hpp:69-78
+
+_F = np.float32
+_libm = C.CDLL(ctypes.util.find_library("m") or "libm.so.6")
+_libm.sinf.restype = _libm.cosf.restype = C.c_float
+_libm.sinf.argtypes = _libm.cosf.argtypes = [C.c_float]
+
+
+def _glm_transform(r, t) -> np.ndarray:
+    """The 4x4 matrix Mesh::apply_transform(r, t) builds (mesh.cpp:652-663), in float32 with glm's operation
+    order: length, the 1e-3 test, angleAxis (sin/cos from the C library's sinf/cosf, as the reference's sincosf)
+    and mat4_cast, then translation in column 3.  Row-major indexing M[row, col]."""
+    r = np.asarray(r, _F).reshape(3)
+    m = np.eye(4, dtype=_F)
+    norm = np.sqrt((r[0] * r[0] + r[1] * r[1]) + r[2] * r[2], dtype=_F)
+    if float(norm) >= 1e-3:
+        ax = r / norm
+        half = _F(norm * _F(0.5))
+        s, w = _F(_libm.sinf(half)), _F(_libm.cosf(half))
+        x, y, z = ax[0] * s, ax[1] * s, ax[2] * s
+        xx, yy, zz, xz, xy, yz, wx, wy, wz = x * x, y * y, z * z, x * z, x * y, y * z, w * x, w * y, w * z
+        one, two = _F(1), _F(2)
+        # glm Result[col][row] -> m[row, col]
+        m[0, 0], m[1, 0], m[2, 0] = one - two * (yy + zz), two * (xy + wz), two * (xz - wy)
+        m[0, 1], m[1, 1], m[2, 1] = two * (xy - wz), one - two * (xx + zz), two * (yz + wx)
+        m[0, 2], m[1, 2], m[2, 2] = two * (xz + wy), two * (yz - wx), one - two * (xx + yy)
+    m[:3, 3] = np.asarray(t, _F).reshape(3)
+    return m
 
 
 def model_matrix(rotation, translation, scale) -> np.ndarray:
@@ -84,6 +114,30 @@ class Mesh:
     def auto_faces(self) -> None:
         """mesh.cpp:628-631."""
         self.faces = np.arange(self.n_verts, dtype=np.uint32)
+
+    def repeat(self, n: int) -> None:
+        """Mesh::repeat (mesh.cpp:633-650): n copies of vert and faces, copy i's indices offset by i * n_verts."""
+        if n < 1:
+            return
+        nv = np.uint32(self.n_verts)
+        faces = np.asarray(self.faces, np.uint32)
+        self.vert = np.tile(np.asarray(self.vert, np.float32), n)
+        self.faces = (np.tile(faces, n) + np.repeat(np.arange(n, dtype=np.uint32) * nv, faces.size)).astype(np.uint32)
+
+    def apply_transform(self, r, t=None, start: int = 0, end: int = -1) -> None:
+        """Mesh::apply_transform (mesh.cpp:652-678) on the host vert, positions only, vertices start..end-1 (end -1:
+        all).  ``r``, ``t``: axis-angle rotation and translation; or ``r`` a 4x4 matrix (M[row, col]) and no ``t``.
+        Bit-exact with glm: each position becomes (M0 x + M1 y) + (M2 z + M3), Mk the matrix's column k."""
+        m = np.asarray(r, _F) if t is None else _glm_transform(r, t)
+        if m.shape != (4, 4):
+            raise ValueError("apply_transform: r must be a 4x4 matrix when t is not given")
+        if end == -1:
+            end = self.n_verts
+        self.vert = np.asarray(self.vert, np.float32)
+        v = self.vert.reshape(-1, VERT_SZ)[start:end]
+        x, y, z = v[:, 0:1], v[:, 1:2], v[:, 2:3]
+        col = [m[:3, k][None, :] for k in range(4)]
+        v[:, :3] = (col[0] * x + col[1] * y) + (col[2] * z + col[3] * _F(1))
 
     def _as_c(self) -> _capi.vr_mesh_desc:
         if self._vert_dev is None:
@@ -154,6 +208,40 @@ class Mesh:
         return m
 
     @staticmethod
+    def Lattice(reso: int = 8, color=GREY) -> "Mesh":
+        """reso^3 unlit points at the cell centres of the unit cube, x slowest (mesh.cpp:493-520)."""
+        c = (np.arange(reso, dtype=_F) + _F(0.5)) / _F(reso)
+        m = Mesh(reso ** 3, 0, 1)
+        v = m.vert.reshape(reso, reso, reso, VERT_SZ)
+        v[..., 0] = c[:, None, None]
+        v[..., 1] = c[None, :, None]
+        v[..., 2] = c[None, None, :]
+        v[..., 3:6] = np.asarray(color, _F)
+        v[..., 6:9] = (1, 0, 0)
+        m.name = "Lattice"
+        m.unlit = True
+        return m
+
+    @staticmethod
+    def CameraFrustum(focal_length, image_width, image_height, z=-0.3, color=GREY) -> "Mesh":
+        """A camera's frustum as 8 unlit lines from the origin to the z plane (mesh.cpp:522-554), in the reference's
+        float operation order, e.g. (z * -halfw) * invf."""
+        invf = _F(1) / _F(focal_length)
+        hw, hh = _F(image_width) * _F(0.5), _F(image_height) * _F(0.5)
+        z = _F(z)
+        col = [float(c) for c in np.asarray(color, _F)]
+        m = Mesh(5, 8, 2)
+        corners = [(-hw, -hh), (-hw, hh), (hw, hh), (hw, -hh)]
+        v = [0.0, 0.0, 0.0, *col, 0.0, 0.0, 1.0]
+        for a, b in corners:
+            v += [(z * a) * invf, (z * b) * invf, z, *col, 0.0, 0.0, 1.0]
+        m.vert = np.asarray(v, _F)
+        m.faces = np.asarray([0, 1, 0, 2, 0, 3, 0, 4, 1, 2, 2, 3, 3, 4, 4, 1], np.uint32)
+        m.name = "CameraFrustum"
+        m.unlit = True
+        return m
+
+    @staticmethod
     def Line(a, b, color=GREY) -> "Mesh":
         """One unlit segment a -> b (mesh.cpp:556-568)."""
         m = Mesh(2, 1, 2)
@@ -196,6 +284,53 @@ class Mesh:
         m.name = "Points"
         m.unlit = True
         return m
+
+
+    # ---- loaders (mesh.cpp:680-951; mesh_io.py)
+    @staticmethod
+    def load_basic_obj(path) -> "Mesh":
+        """Mesh::load_basic_obj: triangles, vertex colours and normals of an OBJ file (see mesh_io.py)."""
+        from .mesh_io import load_basic_obj
+        return load_basic_obj(path)
+
+    @staticmethod
+    def load_mem_basic_obj(text) -> "Mesh":
+        """Mesh::load_mem_basic_obj: :meth:`load_basic_obj` of OBJ text in memory; the mesh is named "OBJ"."""
+        from .mesh_io import load_mem_basic_obj
+        return load_mem_basic_obj(text)
+
+    @staticmethod
+    def open_drawlist(path, default_visible: bool = True) -> list:
+        """Mesh::open_drawlist: the meshes a drawlist .npz file describes, in name order (see mesh_io.py)."""
+        from .mesh_io import open_drawlist
+        return open_drawlist(path, default_visible)
+
+    @staticmethod
+    def open_drawlist_mem(data, default_visible: bool = True) -> list:
+        """Mesh::open_drawlist_mem: :meth:`open_drawlist` of the bytes of a drawlist .npz."""
+        from .mesh_io import open_drawlist_mem
+        return open_drawlist_mem(data, default_visible)
+
+
+def estimate_normals(mesh: Mesh, stream=None) -> None:
+    """estimate_normals (mesh.cpp:63-97) on the GPU: each vertex's normal becomes the normalised sum of the cross
+    products of its triangles (``faces`` empty: consecutive vertex triples), byte for byte the reference's.  Uploads
+    the mesh, runs ``vr_mesh_estimate_normals`` on its device buffer and copies the vertices back, so the host
+    ``vert`` and the device copy both hold the result.  Raises :class:`VolrendError` without a device."""
+    import torch
+    from .host import _stream_ptr
+    faces = np.asarray(mesh.faces, np.uint32).reshape(-1)
+    if not torch.cuda.is_available():
+        check(lib().vr_mesh_estimate_normals(None, 0, None, 0, None))    # VR_ENODEVICE: no CPU fallback
+    mesh.update()
+    vd, fd = mesh._vert_dev, mesh._faces_dev
+    s = torch.cuda.current_stream() if stream is None else stream
+    s.wait_stream(torch.cuda.current_stream())                         # the upload ran on the current stream
+    check(lib().vr_mesh_estimate_normals(vd.data_ptr() if vd.numel() else None, vd.numel() // VERT_SZ,
+                                         fd.data_ptr() if fd is not None else None, faces.size // 3,
+                                         _stream_ptr(s)))
+    s.synchronize()
+    mesh.vert = vd.cpu().numpy()
 
 
 def draw_meshes(cam, meshes, image, depth, stream=None) -> None:
