@@ -42,7 +42,7 @@ $(OBJ)/vr_kernels_%.o: volrend_b200/csrc/vr_kernels_inst.cu volrend_b200/csrc/vr
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -DVR_KBD=$* -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_$*.log || (cat $(OBJ)/ptxas_$*.log; false)
 
-$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h include/volrend_b200.h
+$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -58,6 +58,10 @@ $(OBJ)/vr_normals.o: volrend_b200/csrc/vr_normals.cu volrend_b200/csrc/vr_normal
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_normals.log || (cat $(OBJ)/ptxas_normals.log; false)
 
+$(OBJ)/vr_quant.o: volrend_b200/csrc/vr_quant.cu volrend_b200/csrc/vr_quant.h
+	@mkdir -p $(OBJ)
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_quant.log || (cat $(OBJ)/ptxas_quant.log; false)
+
 $(OBJ)/vr_probe.o: volrend_b200/csrc/vr_probe.cu volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_types.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_probe.log || (cat $(OBJ)/ptxas_probe.log; false)
@@ -70,7 +74,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(CXX) -O3 -std=c++17 -fPIC -Iinclude -c $< -o $@
 
-$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_probe.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
+$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
 oracle: oracle/liboracle.so oracle/libprobe_oracle.so

@@ -298,6 +298,25 @@ int vr_tree_wireframe(const vr_tree* tree, int max_depth, float* vert_dev, int64
 int vr_mesh_estimate_normals(float* vert_dev, int64_t n_verts, const uint32_t* faces_dev, int64_t n_faces,
                              void* stream);
 
+/* ---- tree compression (volrend_b200/csrc/vr_quant.cu) ----------------------------------------------------
+ * Median-cut colour quantisation of a tree into the arrays vr_tree_quant_desc consumes (the format of the
+ * reference's scripts/compress_octree.py, with codebooks always 65536 rows); DESIGN.md section 12 states the
+ * algorithm bit for bit.  data_dev: fp16 [n_child][data_dim], channel-major coefficients (coefficient j of channel
+ * k at k*B + j, B = (data_dim-1)/3), sigma last.  A slot is kept iff sigma > fp16_rn(sigma_thresh), compared as
+ * fp16 (NaN is not kept).  The first n_retain basis functions are copied; each of the other B - n_retain is cut
+ * into 2^bits buckets of its kept slots' RGB triples.  Outputs (device, caller-owned): quant_colors_dev fp16
+ * [B-n_retain][65536][3] (bucket means, +0 for empty buckets and rows >= 2^bits), quant_map_dev u16
+ * [B-n_retain][n_child] (0 for slots not kept), sigma_dev fp16 [n_child] (+0 where not kept), data_retained_dev fp16
+ * [n_retain][n_child][3] (0 where not kept; NULL iff n_retain == 0); *n_kept_out = kept slots.  The kept count
+ * sizes the scratch, so the call synchronises `stream` once; the rest is stream-ordered, with scratch from the
+ * device's default stream-ordered pool (returned to it at the next synchronisation).  VR_EINVAL for bits outside
+ * [1, 16], n_retain < 0, no basis function left to quantise, data_dim != 3B+1, n_child outside [0, INT32_MAX], and,
+ * with no output written, for an Inf / NaN quantised coefficient in a kept slot or more than INT32_MAX points in
+ * all (kept slots x (B - n_retain)). */
+int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim, float sigma_thresh, int32_t n_retain,
+                     int32_t bits, uint16_t* quant_colors_dev, uint16_t* quant_map_dev, uint16_t* sigma_dev,
+                     uint16_t* data_retained_dev, int64_t* n_kept_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

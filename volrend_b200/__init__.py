@@ -9,8 +9,9 @@ from .host import (CAMERA_DEFAULT_FOCAL_LENGTH, VOLREND_GLOBAL_BASIS_MAX, Camera
                    RenderOptions, VolumeRenderer, MultiGpuRenderer, VR_MG_TILES, VR_MG_VIEWS, launch_renderer, render_bands, render_bands_batch, render_batch, render_frames_host, render_frames_png, write_png_file)
 from ._capi import LIB_PATH, VolrendError, lib
 from .mesh import Mesh, draw_meshes, estimate_normals
+from .compress import compress_npz
 
 __all__ = ["N3Tree", "Camera", "RenderOptions", "VolumeRenderer", "DataFormat", "launch_renderer", "MultiGpuRenderer", "VR_MG_VIEWS", "VR_MG_TILES",
-           "Mesh", "draw_meshes", "estimate_normals",
+           "Mesh", "draw_meshes", "estimate_normals", "compress_npz",
            "render_batch", "render_bands", "render_bands_batch", "render_frames_host", "render_frames_png", "write_png_file", "lib", "LIB_PATH", "VolrendError",
            "CAMERA_DEFAULT_FOCAL_LENGTH", "VOLREND_GLOBAL_BASIS_MAX"]

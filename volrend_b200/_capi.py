@@ -122,6 +122,8 @@ SYMBOLS = {
                                  C.c_void_p]),
     "vr_tree_wireframe": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
     "vr_mesh_estimate_normals": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
+    "vr_tree_compress": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
 }
 
 _lib = None

@@ -25,6 +25,7 @@
 #include "vr_kernels.h"
 #include "vr_normals.h"
 #include "vr_probe.h"
+#include "vr_quant.h"
 #include "vr_raster.h"
 #include "vr_types.h"
 #include "vr_wire.h"
@@ -1302,6 +1303,47 @@ int vr_mesh_estimate_normals(float* vert_dev, int64_t n_verts, const uint32_t* f
     g_launches += launches;
     if (e != cudaSuccess)
         return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "mesh normals: %s", cudaGetErrorString(e));
+    return VR_OK;
+}
+
+// Median-cut compression into the quant_colors / quant_map format (kernels: vr_quant.cu).
+int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim, float sigma_thresh, int32_t n_retain,
+                     int32_t bits, uint16_t* quant_colors_dev, uint16_t* quant_map_dev, uint16_t* sigma_dev,
+                     uint16_t* data_retained_dev, int64_t* n_kept_out, void* stream) {
+    if (!n_kept_out) return fail(VR_EINVAL, "null n_kept_out");
+    *n_kept_out = 0;
+    if (bits < 1 || bits > 16) return fail(VR_EINVAL, "bits %d outside [1, 16]", bits);
+    if (n_retain < 0) return fail(VR_EINVAL, "retain %d < 0", n_retain);
+    if (data_dim < 4 || (data_dim - 1) % 3 != 0)
+        return fail(VR_EINVAL, "data_dim %d is not 3 * basis_dim + 1", data_dim);
+    const int basis = (data_dim - 1) / 3, n_quant = basis - n_retain;
+    if (n_quant < 1)
+        return fail(VR_EINVAL, "retain %d leaves no basis function to quantise (the tree has %d)", n_retain, basis);
+    if (n_child < 0 || n_child > INT32_MAX)
+        return fail(VR_EINVAL, "n_child %lld outside [0, %d]", (long long)n_child, INT32_MAX);
+    if ((!data_dev && n_child > 0) || !quant_colors_dev || (!quant_map_dev && n_child > 0) || (!sigma_dev && n_child > 0))
+        return fail(VR_EINVAL, "null argument");
+    if ((n_retain > 0) != (data_retained_dev != nullptr))
+        return fail(VR_EINVAL, "data_retained_dev must be NULL exactly when n_retain == 0");
+    int ndev = 0, dev = -1;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cudaGetDevice(&dev) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
+    }
+    QuantArgs a{};
+    a.data = data_dev; a.n_child = n_child; a.data_dim = data_dim; a.n_retain = n_retain; a.bits = bits;
+    a.thresh = __half2float(__float2half_rn(sigma_thresh));   // sigma > thresh compared as fp16
+    a.colors = quant_colors_dev; a.qmap = quant_map_dev; a.sigma = sigma_dev; a.retained = data_retained_dev;
+    long long kept = 0;
+    int reject = kQuantOk, launches = 0;
+    const cudaError_t e = quant_compress(a, (cudaStream_t)stream, &kept, &reject, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess)
+        return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "tree compress: %s", cudaGetErrorString(e));
+    if (reject == kQuantNonFinite) return fail(VR_EINVAL, "a quantised coefficient of a kept voxel is Inf or NaN");
+    if (reject == kQuantTooManyPoints)
+        return fail(VR_EINVAL, "%lld kept voxels x %d quantised basis functions exceed %d points", kept, n_quant, INT32_MAX);
+    *n_kept_out = kept;
     return VR_OK;
 }
 
