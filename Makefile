@@ -42,7 +42,7 @@ $(OBJ)/vr_kernels_%.o: volrend_b200/csrc/vr_kernels_inst.cu volrend_b200/csrc/vr
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -DVR_KBD=$* -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_$*.log || (cat $(OBJ)/ptxas_$*.log; false)
 
-$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h include/volrend_b200.h
+$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h volrend_b200/csrc/vr_query.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -62,9 +62,13 @@ $(OBJ)/vr_quant.o: volrend_b200/csrc/vr_quant.cu volrend_b200/csrc/vr_quant.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_quant.log || (cat $(OBJ)/ptxas_quant.log; false)
 
-$(OBJ)/vr_probe.o: volrend_b200/csrc/vr_probe.cu volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_types.h include/volrend_b200.h
+$(OBJ)/vr_probe.o: volrend_b200/csrc/vr_probe.cu volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_lumisphere.cuh volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_types.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_probe.log || (cat $(OBJ)/ptxas_probe.log; false)
+
+$(OBJ)/vr_query.o: volrend_b200/csrc/vr_query.cu volrend_b200/csrc/vr_query.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_lumisphere.cuh volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_types.h include/volrend_b200.h
+	@mkdir -p $(OBJ)
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_query.log || (cat $(OBJ)/ptxas_query.log; false)
 
 $(OBJ)/vr_mg.o: volrend_b200/csrc/vr_mg.cu include/volrend_b200.h
 	@mkdir -p $(OBJ)
@@ -74,7 +78,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(CXX) -O3 -std=c++17 -fPIC -Iinclude -c $< -o $@
 
-$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
+$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
 oracle: oracle/liboracle.so oracle/libprobe_oracle.so
@@ -87,6 +91,7 @@ ref:
 	@if [ -d "$(VOLREND_REF)/src/cuda" ]; then $(MAKE) -C oracle -f Makefile.ref VOLREND_REF=$(VOLREND_REF) && \
 	   $(MAKE) -C oracle -f Makefile.wire VOLREND_REF=$(VOLREND_REF) && \
 	   $(MAKE) -C oracle -f Makefile.probe VOLREND_REF=$(VOLREND_REF) && \
+	   $(MAKE) -C oracle -f Makefile.query VOLREND_REF=$(VOLREND_REF) && \
 	   $(MAKE) -C oracle -f Makefile.mesh VOLREND_REF=$(VOLREND_REF); \
 	 else echo "reference tree $(VOLREND_REF) not present: using prebuilt oracle/_ref if any"; fi
 

@@ -195,6 +195,30 @@ int vr_draw_probe(const vr_tree* tree, const vr_camera* cams, int n_views, const
                   const float probe_xyz[3], int disp_size, const vr_rect* tile,
                   uint8_t* rgba8_dev, float* rgba32f_dev, unsigned long long rgba8_surf, void* stream);
 
+/* ---- point queries (volrend_b200/csrc/vr_query.cu) --------------------------------------------------------
+ * query_single_from_root (n3tree_query.hpp:13-48) for n points given in world coordinates (the tree maps them with
+ * offset + scale * xyz, as retrieve_cursor_lumisphere_kernel does, volrend.cu:180-182, and clamps them to
+ * [0, 1-1e-6] with fminf / fmaxf: a NaN coordinate ends up at 1-1e-6).
+ *   data_dev  fp16 [n][data_dim]: the leaf's data row, bit for bit what the reference's `out` points at (colour
+ *             coefficients channel-major, sigma last), or NULL
+ *   cube_dev  float [n]: the reference's cube_sz (N^depth, root children = N), or NULL
+ *   local_dev float [n][3]: the in-cell coordinates the reference leaves in xyz, or NULL
+ * Asynchronous on stream.  VR_EUNSUPPORTED when data_dev != NULL for trees whose basis size keeps only coefficient 0
+ * on the device (the ones vr_probe_lumisphere refuses) or whose data_dim exceeds 3 * basis_dim + 1 (4 for RGBA);
+ * VR_EINVAL for n < 0, NULL xyz_dev with n > 0, or a buffer that is not device memory of the tree's device
+ * (pageable host memory, another device's allocation). */
+int vr_tree_query(const vr_tree* tree, const float* xyz_dev, int64_t n,
+                  uint16_t* data_dev, float* cube_dev, float* local_dev, void* stream);
+
+/* The colour the probe disc of render_kernel gives a leaf seen along dir (volrend.cu:111-128), for n (point,
+ * direction) pairs: rgb_dev float [n][3] = sigmoid(sum over basis_minmax of basis(dir) * coeff) per channel
+ * (SH/SG/ASG), raw RGB for RGBA trees; sigma_dev float [n] = the leaf's sigma.  Directions are used as given (not
+ * normalised, as the probe uses the rotated unit vector).  Of opt only basis_minmax is read, clamped as vr_draw_probe
+ * clamps it (opt NULL: the whole basis).  Either output may be NULL.  VR_EUNSUPPORTED when rgb_dev != NULL for the
+ * trees vr_probe_lumisphere refuses; VR_EINVAL as vr_tree_query, and for NULL dir_dev with rgb_dev and n > 0. */
+int vr_tree_eval(const vr_tree* tree, const float* xyz_dev, const float* dir_dev, int64_t n,
+                 const vr_options* opt, float* rgb_dev, float* sigma_dev, void* stream);
+
 /* Diagnostics: one full-frame render with the instrumented kernel that also records, per 8x4-pixel
  * work item (row-major tiles of 8x4), {start ns, end ns, SM id, global warp id} into
  * trace_dev[4 * n_items] (n_items = ceil(w/8)*ceil(h/4)). */

@@ -14,6 +14,9 @@ built from the reference sources by oracle/Makefile.ref).  Needs a GPU.
   python tools/make_golden.py --mesh OUT         tests/golden/ref/mesh_*.npz, Mesh::open_drawlist_mem and
                                                  Mesh::load_mem_basic_obj of the inputs of tests/mesh_io_cases.py
                                                  (needs only oracle/_ref/libref_mesh.so, no GPU)
+  python tools/make_golden.py --query OUT        tests/golden/ref/query_*.npz, the reference's query_single_from_root
+                                                 (oracle/_ref/libref_query.so) on the trees and point sets of
+                                                 tests/query_cases.py
 
 OUT receives the files; copy them to tests/golden/ (or tests/golden/ref/) and commit them.
 """
@@ -147,8 +150,38 @@ def mesh_loads(out_dir, only, tmpdir):
             print(name, "vertices", rec["m0_vert"].size // 9, flush=True)
 
 
+def queries(out_dir, only, tmpdir):
+    import query_cases as qc
+    from oracle import ref_query
+    for name in qc.QUERY_TREES:
+        if only and name not in only:
+            continue
+        z = qc.query_tree(name)
+        path = os.path.join(tmpdir, name + ".npz")
+        np.savez(path, **z)
+        rt = ref_query.RefQueryTree(path)
+        pts, lab = qc.all_points(name, z)
+        data, cube, local, _ = rt.query(pts)
+        rt.close()
+        os.remove(path)
+        np.savez_compressed(os.path.join(out_dir, os.path.basename(qc.golden_path(name))), case=np.array(name),
+                            points=pts, set=lab, data=data.view(np.uint16), cube=cube, local=local)
+        print(name, "points", len(pts), "data_dim", data.shape[1], "max cube", float(cube.max()), flush=True)
+
+
 def main():
     args = sys.argv[1:]
+    if "--query" in args:
+        from oracle import ref_query
+        args = [a for a in args if a != "--query"]
+        if not args:
+            raise SystemExit(__doc__)
+        if not ref_query.available():
+            raise SystemExit(f"{ref_query.LIB_PATH} is missing: build it with `make ref` where the reference sources are")
+        os.makedirs(args[0], exist_ok=True)
+        with tempfile.TemporaryDirectory() as tmpdir:
+            queries(args[0], args[1:], tmpdir)
+        return
     if "--mesh" in args:                # CPU only: the reference's Mesh loaders
         from oracle import ref_mesh
         args = [a for a in args if a != "--mesh"]

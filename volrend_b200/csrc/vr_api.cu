@@ -26,6 +26,7 @@
 #include "vr_normals.h"
 #include "vr_probe.h"
 #include "vr_quant.h"
+#include "vr_query.h"
 #include "vr_raster.h"
 #include "vr_types.h"
 #include "vr_wire.h"
@@ -387,13 +388,6 @@ __global__ void queue_init_kernel(unsigned char* slots) {
     if (i < 2) reinterpret_cast<unsigned int*>(slot)[i] = 0u;
     reinterpret_cast<unsigned long long*>(slot + kQueueStateOff)[i] = ((unsigned long long)kBlkInvalid << 32) | kBlkIdle;
     reinterpret_cast<unsigned int*>(slot + kQueueLockOff)[i] = 0u;
-}
-
-// retrieve_cursor_lumisphere_kernel (volrend.cu:175-191): descends the wide tables.
-__global__ void probe_kernel(TreeDev tree, float x, float y, float z, int n_out, float* __restrict__ out) {
-    const uint32_t eidx = probe_leaf_entry(tree, x, y, z);
-    const unsigned short* rec = reinterpret_cast<const unsigned short*>(tree.wrecs + (size_t)eidx * tree.rec_bytes);
-    for (int i = threadIdx.x; i < n_out; i += blockDim.x) out[i] = __half2float(__ushort_as_half(rec[i]));
 }
 
 }  // namespace
@@ -1104,9 +1098,93 @@ int vr_probe_lumisphere(const vr_tree* t, const float xyz[3], float* out_dev, vo
     // the resident record holds the colour coefficients only: 3 per RGBA leaf, 3*basis_dim otherwise
     // (extra trailing channels of an over-wide data_dim are not kept)
     const int resident = t->dev.kbd < 0 ? 3 : 3 * t->dev.kbd;
-    const int n_out = t->data_dim - 1 < resident ? t->data_dim - 1 : resident;
-    probe_kernel<<<1, 32, 0, (cudaStream_t)stream_>>>(t->dev, xyz[0], xyz[1], xyz[2], n_out, out_dev);
-    VR_CUDA(cudaGetLastError());
+    QueryLaunch Q{};
+    Q.tree = t->dev;
+    Q.n = 1;
+    for (int i = 0; i < 3; ++i) Q.point[i] = xyz[i];
+    Q.coef = out_dev;
+    Q.n_coef = t->data_dim - 1 < resident ? t->data_dim - 1 : resident;
+    VR_CUDA(query_launch(Q, t->dev.kbd, false, t->num_sms, (cudaStream_t)stream_));
+    g_launches += 1;
+    return VR_OK;
+}
+
+// Checks shared by vr_tree_query and vr_tree_eval; *full: the device keeps the tree's whole data row (every colour
+// coefficient, and no halves between them and sigma that the records drop).
+static int query_check(const vr_tree* t, const float* xyz, int64_t n, bool* full) {
+    if (!t) return fail(VR_EINVAL, "null tree");
+    if (n < 0) return fail(VR_EINVAL, "n = %lld < 0", (long long)n);
+    if (!xyz && n > 0) return fail(VR_EINVAL, "null points with n = %lld", (long long)n);
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) return fail(VR_ENODEVICE, "no CUDA device");
+    if (dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
+    const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
+    *full = !(t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim) && t->data_dim == 3 * nb + 1;
+    return VR_OK;
+}
+
+// The kernel dereferences `p`: it must be memory the tree's device can address (not pageable host memory, not
+// another device's allocation).
+static int query_buffer_check(const vr_tree* t, const void* p, const char* what) {
+    if (!p) return VR_OK;
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(VR_EINVAL, "%s is not a CUDA allocation", what);
+    }
+    if (a.type == cudaMemoryTypeUnregistered) return fail(VR_EINVAL, "%s is not device memory", what);
+    if (a.type == cudaMemoryTypeDevice && a.device != t->device)
+        return fail(VR_EINVAL, "%s lives on device %d, the tree on device %d", what, a.device, t->device);
+    return VR_OK;
+}
+
+// query_single_from_root (n3tree_query.hpp:13-48) for n world points (kernel: vr_query.cu).
+int vr_tree_query(const vr_tree* t, const float* xyz_dev, int64_t n, uint16_t* data_dev, float* cube_dev,
+                  float* local_dev, void* stream_) {
+    bool full = false;
+    const int rc = query_check(t, xyz_dev, n, &full);
+    if (rc) return rc;
+    if (data_dev && !full)
+        return fail(VR_EUNSUPPORTED, "data rows unavailable for basis_dim %d, data_dim %d (the device keeps %s)",
+                    t->dev.basis_dim, t->data_dim, t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim
+                    ? "only coefficient 0" : "the colour coefficients and sigma only");
+    if (n == 0 || (!data_dev && !cube_dev && !local_dev)) return VR_OK;
+    int bc;
+    if ((bc = query_buffer_check(t, xyz_dev, "xyz_dev")) || (bc = query_buffer_check(t, data_dev, "data_dev")) ||
+        (bc = query_buffer_check(t, cube_dev, "cube_dev")) || (bc = query_buffer_check(t, local_dev, "local_dev")))
+        return bc;
+    QueryLaunch Q{};
+    Q.tree = t->dev;
+    Q.xyz = xyz_dev; Q.n = n;
+    Q.data = data_dev; Q.cube = cube_dev; Q.local = local_dev;
+    VR_CUDA(query_launch(Q, t->dev.kbd, false, t->num_sms, (cudaStream_t)stream_));
+    g_launches += 1;
+    return VR_OK;
+}
+
+// The probe disc's colour (volrend.cu:111-128) of the leaves of n world points along n directions (kernel: vr_query.cu).
+int vr_tree_eval(const vr_tree* t, const float* xyz_dev, const float* dir_dev, int64_t n, const vr_options* opt,
+                 float* rgb_dev, float* sigma_dev, void* stream_) {
+    bool full = false;
+    const int rc = query_check(t, xyz_dev, n, &full);
+    if (rc) return rc;
+    if (rgb_dev && !dir_dev && n > 0) return fail(VR_EINVAL, "null directions with n = %lld", (long long)n);
+    if (rgb_dev && t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim)
+        return fail(VR_EUNSUPPORTED, "eval unavailable for basis_dim %d (only coefficient 0 is resident)", t->dev.basis_dim);
+    if (n == 0 || (!rgb_dev && !sigma_dev)) return VR_OK;
+    int bc;
+    if ((bc = query_buffer_check(t, xyz_dev, "xyz_dev")) || (rgb_dev && (bc = query_buffer_check(t, dir_dev, "dir_dev"))) ||
+        (bc = query_buffer_check(t, rgb_dev, "rgb_dev")) || (bc = query_buffer_check(t, sigma_dev, "sigma_dev")))
+        return bc;
+    QueryLaunch Q{};
+    Q.tree = t->dev;
+    Q.xyz = xyz_dev; Q.dir = dir_dev; Q.n = n;
+    Q.rgb = rgb_dev; Q.sigma = sigma_dev;
+    // as vr_draw_probe: basis_minmax clamped to the tree's basis (NULL opt: the whole basis)
+    const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
+    Q.bmin = opt ? std::max(opt->basis_minmax[0], 0) : 0;
+    Q.bmax = opt ? std::min(opt->basis_minmax[1], nb - 1) : nb - 1;
+    VR_CUDA(query_launch(Q, t->dev.kbd, true, t->num_sms, (cudaStream_t)stream_));
     g_launches += 1;
     return VR_OK;
 }

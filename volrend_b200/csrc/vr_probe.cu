@@ -13,30 +13,11 @@
 // The integer candidate test wraps like the 32-bit adds of the SASS.
 #include <cuda_runtime.h>
 
-#include "vr_march.cuh"
+#include "vr_lumisphere.cuh"
 #include "vr_probe.h"
 
 namespace vrb {
 namespace {
-
-// maybe_precalc_basis (lumisphere.hpp:9-87) as render_kernel's disc instance computes it.  It is the march's basis
-// (sh_basis / sg_basis) except for one contraction: this instance fuses -y*y into 4zz - xx - yy (B[11], B[13]).
-template <int KBD>
-__device__ __forceinline__ void disc_basis(const TreeDev& tree, float x, float y, float z,
-                                           float (&B)[BasisCount<KBD>::n]) {
-    if (tree.format == VR_FMT_SH) {
-        sh_basis<KBD>(x, y, z, B);
-        if constexpr (KBD >= 16) {
-            const float z4 = __fmaf_rn(-y, y, __fmaf_rn(__fmul_rn(z, z), 4.f, -__fmul_rn(x, x)));
-            B[11] = (float)__dmul_rn(__dmul_rn((double)y, -0.4570457994644658), (double)z4);
-            B[13] = (float)__dmul_rn((double)z4, __dmul_rn((double)x, -0.4570457994644658));
-        }
-    } else {
-#pragma unroll
-        for (int i = 0; i < BasisCount<KBD>::n; ++i) B[i] = 0.f;
-        sg_basis<KBD>(tree, x, y, z, B);
-    }
-}
 
 template <int KBD>
 __global__ void __launch_bounds__(256) probe_disc_kernel(const ProbeLaunch P) {
@@ -62,28 +43,15 @@ __global__ void __launch_bounds__(256) probe_disc_kernel(const ProbeLaunch P) {
     const float c = __fmaf_rn(a, a, __fmul_rn(b, b));
     if (!(c <= 1.f)) return;  // marched normally: the frame already holds it
 
-    float out[3];
-    if constexpr (KBD < 0) {
-        out[0] = s_coef[0]; out[1] = s_coef[1]; out[2] = s_coef[2];
-    } else {
+    float d[3] = {0.f, 0.f, 0.f};
+    if constexpr (KBD >= 0) {
         const float s = __fsqrt_rn(__fsub_rn(1.f, c));
         const float* m = cam.c2w;
-        float d[3];
 #pragma unroll
         for (int k = 0; k < 3; ++k) d[k] = __fmaf_rn(-m[6 + k], s, __fmaf_rn(b, m[3 + k], -__fmul_rn(a, m[k])));
-        float B[BasisCount<KBD>::n];
-        disc_basis<KBD>(P.tree, d[0], d[1], d[2], B);
-#pragma unroll
-        for (int t = 0; t < 3; ++t) {
-            float tmp = 0.f;
-#pragma unroll
-            for (int j = 0; j < BasisCount<KBD>::n; ++j)
-                if (j >= P.bmin && j <= P.bmax) tmp = __fmaf_rn(s_coef[t * KBD + j], B[j], tmp);
-            float e, sc;
-            expf_parts(-tmp, e, sc);
-            out[t] = __frcp_rn(__fmaf_rn(sc, e, 1.f));
-        }
     }
+    float out[3];
+    lumisphere_rgb<KBD>(P.tree, d[0], d[1], d[2], P.bmin, P.bmax, [&](int k) { return s_coef[k]; }, out);
     // volrend.cu:153-163 with alpha 1: the background or existing colour enters with weight 0
     float o[4] = {__fadd_rn(out[0], 0.f), __fadd_rn(out[1], 0.f), __fadd_rn(out[2], 0.f), 1.f};
     const uint32_t q = quantise(o);

@@ -87,6 +87,7 @@ class N3Tree:
         self.child_ = None      # int32 [cap,N,N,N]
         self.extra_ = None      # f32
         self._handle = None     # vr_tree*
+        self._device = None     # CUDA device of the tree (set by load_cuda)
         self._data_loaded = False
         self._cuda_loaded = False
         if path is not None:
@@ -253,6 +254,8 @@ class N3Tree:
             check(lib().vr_tree_create(C.byref(d), C.byref(h)))
         self._handle = h
         self._cuda_loaded = True
+        import torch
+        self._device = torch.cuda.current_device()     # the device vr_tree_create put the tree on
 
     def _plain_desc(self):
         """vr_tree_desc over the decoded host arrays (keeps them alive through the returned tuple)."""
@@ -298,6 +301,95 @@ class N3Tree:
         segments, 12 per cell = 24 vertices of 9 float32 (position, colour 0, normal 0,0,1).  Generated on the GPU
         from the device tree and copied to the host."""
         return self.wireframe_device(max_depth).cpu().numpy()
+
+    # -- point queries (vr_tree_query / vr_tree_eval)
+    def _check_points(self, name: str, pts, n=None) -> bool:
+        """Validates a ``[n, 3]`` float32 numpy array or CUDA tensor; True for numpy."""
+        import torch
+        if self.child_ is None:
+            raise RuntimeError("N3Tree has no data: open a tree first")
+        is_np = isinstance(pts, np.ndarray)
+        if not is_np and not (isinstance(pts, torch.Tensor) and pts.is_cuda):
+            raise TypeError(f"{name} must be a float32 numpy array or a CUDA torch tensor")
+        if pts.dtype not in (np.float32, torch.float32):
+            raise TypeError(f"{name} must be float32, not {pts.dtype}")
+        if pts.ndim != 2 or pts.shape[1] != 3 or (n is not None and pts.shape[0] != n):
+            raise ValueError(f"{name} must have shape [{'n' if n is None else n}, 3], not {tuple(pts.shape)}")
+        return is_np
+
+    def _launch(self, inputs, outputs, stream, call) -> None:
+        """Runs ``call(stream_ptr)`` on ``stream`` (None: torch's current stream) on the tree's device, ordered after
+        the work of the current stream that produced ``inputs`` and allocated ``outputs``; the tensors are recorded
+        on ``stream`` so that the caching allocator does not hand their memory out while the kernel still runs."""
+        import torch
+        with torch.cuda.device(self._device):
+            cur = torch.cuda.current_stream()
+            if stream is None:
+                s = cur
+            elif isinstance(stream, torch.cuda.Stream):
+                s = stream
+            else:
+                s = torch.cuda.ExternalStream(int(stream))
+            if s != cur:
+                s.wait_stream(cur)
+                for t in (*inputs, *outputs):
+                    t.record_stream(s)
+            call(_stream_ptr(s))
+        return s
+
+    def _on_device(self, name: str, pts):
+        """Loads the tree onto the GPU if needed; -> contiguous CUDA float32 tensor of ``pts`` on the tree's device."""
+        import torch
+        if not self.is_cuda_loaded():
+            self.load_cuda()
+        if isinstance(pts, np.ndarray):
+            return torch.from_numpy(np.ascontiguousarray(pts)).to(torch.device("cuda", self._device))
+        if pts.device.index != self._device:
+            raise ValueError(f"{name} live on {pts.device}, the tree on cuda:{self._device}")
+        with torch.cuda.device(self._device):
+            return pts.contiguous()
+
+    def query(self, points, *, stream=None):
+        """query_single_from_root for world points ``[n, 3]`` float32 -> ``(data, cube_sz, local)``: the leaf's data
+        row (float16 ``[n, data_dim]``, sigma last), its cube size N^depth (float32 ``[n]``) and the point's in-cell
+        coordinates (float32 ``[n, 3]``).  numpy in, numpy out: the call returns when the results are on the host.  A
+        CUDA tensor (on the tree's device) in gives tensors on that device, written on ``stream`` (default: the
+        current stream) after the current stream's earlier work, with no host round trip."""
+        import torch
+        is_np = self._check_points("points", points)
+        x = self._on_device("points", points)
+        n = x.shape[0]
+        data = torch.empty((n, self.data_dim), dtype=torch.float16, device=x.device)
+        cube = torch.empty(n, dtype=torch.float32, device=x.device)
+        local = torch.empty((n, 3), dtype=torch.float32, device=x.device)
+        s = self._launch((x,), (data, cube, local), stream,
+                         lambda sp: check(lib().vr_tree_query(self._handle, x.data_ptr(), n, data.data_ptr(),
+                                                              cube.data_ptr(), local.data_ptr(), sp)))
+        if is_np:
+            s.synchronize()
+            return data.cpu().numpy(), cube.cpu().numpy(), local.cpu().numpy()
+        return data, cube, local
+
+    def eval(self, points, dirs, options=None, *, stream=None):
+        """The probe disc's colour of the leaves of world points ``[n, 3]`` seen along ``dirs`` ``[n, 3]`` (used as
+        given) -> ``(rgb, sigma)`` float32 ``[n, 3]`` and ``[n]``; of ``options`` (a :class:`RenderOptions`) only
+        ``basis_minmax`` is read.  Same input and output types, devices and stream order as :meth:`query`."""
+        import torch
+        is_np = self._check_points("points", points)
+        if self._check_points("dirs", dirs, points.shape[0]) != is_np:
+            raise TypeError("points and dirs must both be numpy arrays or both CUDA tensors")
+        x, d = self._on_device("points", points), self._on_device("dirs", dirs)
+        n = x.shape[0]
+        rgb = torch.empty((n, 3), dtype=torch.float32, device=x.device)
+        sigma = torch.empty(n, dtype=torch.float32, device=x.device)
+        o = (options if options is not None else RenderOptions())._as_c()
+        s = self._launch((x, d), (rgb, sigma), stream,
+                         lambda sp: check(lib().vr_tree_eval(self._handle, x.data_ptr(), d.data_ptr(), n, C.byref(o),
+                                                             rgb.data_ptr(), sigma.data_ptr(), sp)))
+        if is_np:
+            s.synchronize()
+            return rgb.cpu().numpy(), sigma.cpu().numpy()
+        return rgb, sigma
 
     def info(self) -> dict:
         inf = _capi.vr_tree_info()
