@@ -17,6 +17,8 @@
  *                                      colour + depth inputs (volrend.cu:92-96,143-146)
  *   vr_render_batch                    the per-pose loop of main_headless.cpp:208-223 as
  *                                      one call (same per-view semantics)
+ *   vr_render_batch_opts               the same with one RenderOptions per view (the frames of
+ *                                      main_anim.cpp:1252-1262, whose options change per frame)
  *   vr_render_frames_host              main_headless.cpp:208-223 with `-o`: renders and
  *                                      copies every frame to host memory (:216-219)
  *   vr_probe_lumisphere                retrieve_cursor_lumisphere_kernel (volrend.cu:175-191)
@@ -140,6 +142,16 @@ int vr_render_batch(const vr_tree* tree, const vr_camera* cams, int n_views, con
                     const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev,
                     vr_counters* counters_dev, void* stream);
 
+/* Same, with options per view: view i is rendered with opts[i] (n_views entries), as vr_render would render it.
+ * Output layout, tile, counters, the one-image-size rule and the splitting of very large batches are those of
+ * vr_render_batch; NULL opts with n_views > 0 is VR_EINVAL.  The options travel through a device ring beside the
+ * camera ring (allocated by the first such call on a (tree, stream)).  Batches of two or more views run on the
+ * inline-shading (3 + 16*193) or shading-queue (7) kernel; any other vr_set_variant setting is VR_EUNSUPPORTED.
+ * Used by the animator (volrend_anim, main_anim.cpp:268-307), whose interpolated options change every frame. */
+int vr_render_batch_opts(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opts,
+                         const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev,
+                         void* stream);
+
 /* launch_renderer(offscreen=false): rgba8_dev is read (existing colour) and overwritten;
  * depth_dev holds the per-pixel ray-distance limit (world units), both tile-sized. */
 int vr_render_composite(const vr_tree* tree, const vr_camera* cam, const vr_options* opt,
@@ -174,6 +186,9 @@ int vr_render_frames_host(const vr_tree* tree, const vr_camera* cams, int n_view
 int vr_write_png(const char* path, const uint8_t* rgba8_host, int width, int height);
 int vr_render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
                          const char* const* paths, int n_threads);
+/* The same pipeline with options per view (opts[i] for view i, as vr_render_batch_opts). */
+int vr_render_frames_png_opts(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opts,
+                              const char* const* paths, int n_threads);
 
 /* Copies the colour coefficients of the leaf containing world point xyz into out_dev as floats
  * (retrieve_cursor_lumisphere_kernel): min(data_dim-1, 3*basis_dim) values (3 for RGBA). */

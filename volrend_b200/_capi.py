@@ -75,6 +75,8 @@ SYMBOLS = {
                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_render_batch": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
                                   C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vr_render_batch_opts": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
+                                       C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_render_composite": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.POINTER(vr_options),
                                       C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_render_surface": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.POINTER(vr_options),
@@ -84,6 +86,8 @@ SYMBOLS = {
     "vr_write_png": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int, C.c_int]),
     "vr_render_frames_png": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
                                        C.POINTER(C.c_char_p), C.c_int]),
+    "vr_render_frames_png_opts": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
+                                            C.POINTER(C.c_char_p), C.c_int]),
     "vr_probe_lumisphere": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_void_p, C.c_void_p]),
     "vr_tree_query": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_tree_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(vr_options), C.c_void_p,

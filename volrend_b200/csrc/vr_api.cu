@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "volrend_b200.h"
+#include "vr_frames.h"
 #include "vr_kernels.h"
 #include "vr_normals.h"
 #include "vr_probe.h"
@@ -77,6 +78,8 @@ int rec_bytes_for(int kbd) { return kbd <= 1 ? 8 : ((3 * kbd * 2 + 15) / 16) * 1
 struct StreamRes {
     unsigned int* queues = nullptr;  // kQueueSlots slots of kQueueSlotBytes: {head, done}, per-SM block states and locks (vr_march.cuh)
     CamDev* cam_ring = nullptr;      // kCamRing entries; batches take consecutive slots
+    OptDev* opt_ring = nullptr;      // kCamRing entries beside cam_ring (same slots), allocated by the first
+                                     // batch with options per view
     unsigned int next_queue = 0, cam_pos = 0;
     unsigned char* pool = nullptr;   // parked-ray stacks of the ray-pool kernel (kind 8), allocated on first use
     size_t pool_bytes = 0;
@@ -448,7 +451,7 @@ void vr_tree_destroy(vr_tree* t) {
     cudaSetDevice(t->device);
     cudaFree(t->nodes); cudaFree(t->recs); cudaFree(t->top); cudaFree(t->extra);
     cudaFree(t->wide); cudaFree(t->wslot); cudaFree(t->wrecs);
-    for (auto& kv : t->res) { cudaFree(kv.second.queues); cudaFree(kv.second.cam_ring); cudaFree(kv.second.pool); }
+    for (auto& kv : t->res) { cudaFree(kv.second.queues); cudaFree(kv.second.cam_ring); cudaFree(kv.second.opt_ring); cudaFree(kv.second.pool); }
     for (int i = 0; i < vr_tree::HostPath::kRing; ++i) {
         cudaFree(t->host.buf[i]);
         if (t->host.rendered[i]) cudaEventDestroy(t->host.rendered[i]);
@@ -815,7 +818,10 @@ namespace {
 // Cameras of a batch go through a device ring owned by (tree, stream): no allocation on the launch path (a
 // stream-ordered pool would hand memory back to the OS at every synchronisation), and a slot is rewritten
 // only by a copy that is stream-ordered behind the launch that read it.  n_views <= kCamRing.
-int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_t stream, LaunchDev& P) {
+// opts != nullptr: n_views options, one per view, staged the same way into the option ring, slot for slot beside
+// the cameras (the ring is allocated here on first use: callers that never pass per-view options pay nothing).
+int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_t stream, LaunchDev& P,
+               const vr_options* opts = nullptr) {
     if (n_views <= 1) return VR_OK;
     vr_tree* mt = const_cast<vr_tree*>(t);
     StreamRes* sr = nullptr;
@@ -823,6 +829,7 @@ int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_
     unsigned int slot;
     {
         std::lock_guard<std::mutex> lk(mt->res_mu);
+        if (opts && !sr->opt_ring) VR_CUDA(cudaMalloc(&sr->opt_ring, kCamRing * sizeof(OptDev)));
         if (sr->cam_pos + (unsigned int)n_views > (unsigned int)kCamRing) sr->cam_pos = 0;  // no wrap inside a batch
         slot = sr->cam_pos;
         sr->cam_pos += (unsigned int)n_views;
@@ -833,14 +840,23 @@ int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_
     VR_CUDA(cudaMemcpyAsync(dcams, h.data(), sizeof(CamDev) * n_views, cudaMemcpyHostToDevice, stream));
     // pageable source: the copy has been staged when cudaMemcpyAsync returns
     P.cams = dcams;
+    if (opts) {
+        std::vector<OptDev> ho(n_views);
+        for (int i = 0; i < n_views; ++i) fill_opt(ho[i], &opts[i]);
+        OptDev* dopts = sr->opt_ring + slot;
+        VR_CUDA(cudaMemcpyAsync(dopts, ho.data(), sizeof(OptDev) * n_views, cudaMemcpyHostToDevice, stream));
+        P.opts = dopts;
+    }
     return VR_OK;
 }
 }  // namespace
 
-extern "C" {
+namespace vrb {
 
-int vr_render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, const vr_rect* tile,
-                    uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream_) {
+// vr_render_batch (opt_stride 0: one options struct for every view) and vr_render_batch_opts (opt_stride 1: view i
+// uses opt[i]).  A batch of one view is an ordinary single-view launch with that view's options.
+int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
+                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
     if (n_views == 0) return VR_OK;
@@ -850,6 +866,13 @@ int vr_render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const 
     for (int i = 1; i < n_views; ++i)
         if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
             return fail(VR_EINVAL, "all views of a batch must share one image size");
+    const bool per_view = opt_stride != 0 && n_views > 1;
+    if (per_view) {
+        // the per-view kernels are instantiated for the two product kernels (inline shading, shading queue) only
+        const int v = vr_get_variant();
+        if (v != 0 && v != kVariantQueue && v != kVariantInline)
+            return fail(VR_EUNSUPPORTED, "kernel variant %d has no per-view options form", v);
+    }
     if (r.w == 0 || r.h == 0) return VR_OK;
     LaunchDev P{};
     P.tree = t->dev;
@@ -865,14 +888,30 @@ int vr_render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const 
         const size_t tile_px = (size_t)r.w * r.h;
         for (int v0 = 0; v0 < n_views; v0 += max_views) {
             const int nv = n_views - v0 < max_views ? n_views - v0 : max_views;
-            rc = vr_render_batch(t, cams + v0, nv, opt, tile, rgba8_dev ? rgba8_dev + 4 * tile_px * v0 : nullptr,
-                                 rgba32f_dev ? rgba32f_dev + 4 * tile_px * v0 : nullptr, counters_dev, stream_);
+            rc = render_batch(t, cams + v0, nv, opt + (size_t)opt_stride * v0, opt_stride, tile,
+                              rgba8_dev ? rgba8_dev + 4 * tile_px * v0 : nullptr,
+                              rgba32f_dev ? rgba32f_dev + 4 * tile_px * v0 : nullptr, counters_dev, stream_);
             if (rc) return rc;
         }
         return VR_OK;
     }
-    if ((rc = stage_cams(t, cams, n_views, stream, P))) return rc;
+    if ((rc = stage_cams(t, cams, n_views, stream, P, per_view ? opt : nullptr))) return rc;
     return dispatch(t, P, counters_dev != nullptr, false, stream);
+}
+
+}  // namespace vrb
+
+extern "C" {
+
+int vr_render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, const vr_rect* tile,
+                    uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream) {
+    return render_batch(t, cams, n_views, opt, 0, tile, rgba8_dev, rgba32f_dev, counters_dev, stream);
+}
+
+int vr_render_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opts,
+                         const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev,
+                         void* stream) {
+    return render_batch(t, cams, n_views, opts, 1, tile, rgba8_dev, rgba32f_dev, counters_dev, stream);
 }
 
 int vr_render_bands_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int band_h,
@@ -987,8 +1026,10 @@ int vr_render_surface(const vr_tree* t, const vr_camera* cam, const vr_options* 
     return dispatch(t, P, false, true, (cudaStream_t)stream_);
 }
 
-int vr_render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
-                          uint8_t* rgba8_host) {
+}  // extern "C"
+
+int vrb::render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
+                            int opt_stride, uint8_t* rgba8_host) {
     // main_headless.cpp:208-223 with -o: every frame goes back to host memory.  Frames are
     // rendered in chunks of a few views per launch on two alternating streams (the tail of
     // one chunk overlaps the head of the next) and copied out on a third stream while the
@@ -1032,7 +1073,8 @@ int vr_render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views, 
         const int s = c % kRing;
         cudaStream_t sr = R.sr[c & 1];
         if (c >= kRing) VR_CUDA(cudaStreamWaitEvent(sr, R.copied[s], 0));
-        rc = vr_render_batch(t, cams + v0, nv, opt, nullptr, R.buf[s], nullptr, nullptr, sr);
+        rc = render_batch(t, cams + v0, nv, opt + (size_t)opt_stride * v0, opt_stride, nullptr, R.buf[s], nullptr,
+                          nullptr, sr);
         if (rc) return rc;
         VR_CUDA(cudaEventRecord(R.rendered[s], sr));
         VR_CUDA(cudaStreamWaitEvent(R.sc, R.rendered[s], 0));
@@ -1043,6 +1085,13 @@ int vr_render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views, 
     VR_CUDA(cudaStreamSynchronize(R.sr[0]));
     VR_CUDA(cudaStreamSynchronize(R.sr[1]));
     return VR_OK;
+}
+
+extern "C" {
+
+int vr_render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
+                          uint8_t* rgba8_host) {
+    return render_frames_host(t, cams, n_views, opt, 0, rgba8_host);
 }
 
 int vr_dev_alloc(size_t bytes, void** ptr) {

@@ -7,6 +7,8 @@
 //   kind 8           (VR_EXPERIMENTS) the same kernel with the ray pool (POOL = true): measured, slower
 //   kind 3, tune 193 march_persistent_kernel with inline shading: default for batches and for RGBA / 1 / 25 basis
 //                    functions, and the A/B partner of the queue kernel in the parity tests and the bench
+// Both also come as kOutViewOpts instantiations (plain and counting), which read each view's options from
+// LaunchDev::opts: batches with options per view.
 // Built only with -DVR_EXPERIMENTS (make lib SUFFIX=_exp EXTRA=-DVR_EXPERIMENTS): the measured and
 // rejected structures of round 1 -- CTA-per-tile kernel, TMA-staged top grid, deferred shading,
 // software-pipelined march, tuning knobs (DESIGN.md 4).
@@ -182,6 +184,14 @@ cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg) {
     if (variant == 0) variant = (P.n_views == 1 && KBD >= 4 && KBD <= 16) ? 7 : 3 + 16 * kInline;
     const int kind = variant & 15, tune = variant >> 4;
     const bool queue = kind == 7 || kind == 8;
+    if (P.opts) {   // options per view (vr_render_batch_opts): instantiated for the two product kernels only
+        if (cfg.surface || !(kind == 7 || (kind == 3 && tune == kInline))) return cudaErrorInvalidValue;
+        if (cfg.count)
+            return queue ? launch_queue<KBD, true, kOutViewOpts>(P, cfg)
+                         : launch_persistent<KBD, false, true, kOutViewOpts, kInline>(P, cfg);
+        return queue ? launch_queue<KBD, false, kOutViewOpts>(P, cfg)
+                     : launch_persistent<KBD, false, false, kOutViewOpts, kInline>(P, cfg);
+    }
 #ifdef VR_EXPERIMENTS
     if (kind == 8) {   // measured and rejected (DESIGN.md 4): the ray-pool form of the queue kernel
         if (cfg.surface) return launch_queue<KBD, false, kOutSurface, true>(P, cfg);

@@ -270,7 +270,11 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) march_queue_kernel(const _
         pdl_wait_predecessor();
         dep_done = true;
     }
-    const float step = P.opt.step_size, sthr = P.opt.sigma_thresh;
+    float step = P.opt.step_size, sthr = P.opt.sigma_thresh;
+    // kOutViewOpts: the options of the view of the warp's current work item (read when the item is taken, and again
+    // for the pixel write, so that only the loop constants stay live across the march)
+    OptDev vopt{};
+    const OptDev& opt = OUT == kOutViewOpts ? vopt : P.opt;
     const uint32_t* __restrict__ wide = P.tree.wide;
     const int wp = P.tree.wide_p;
 
@@ -355,6 +359,10 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) march_queue_kernel(const _
             const int lx = tx * kTW + (lane % kTW), ly = ty * kTH + (lane / kTW);
             const bool inb = lx < P.w && ly < P.h;
             const CamDev& cam = P.cams ? P.cams[view] : P.cam;
+            if constexpr (OUT == kOutViewOpts) {
+                vopt = P.opts[view];
+                step = vopt.step_size; sthr = vopt.sigma_thresh;
+            }
             if (COUNT && P.trace) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_begin));
 
             const int px = P.x0 + lx, py = P.y0 + frame_row(P, ly);
@@ -372,10 +380,10 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) march_queue_kernel(const _
             }
             if (inb && P.tree.N > 0) {
                 float vd[3];
-                hit = ray_geometry(P.tree, P.opt, cam, px, py, tlim, R, vd, P.tree.pos_scale);
+                hit = ray_geometry(P.tree, opt, cam, px, py, tlim, R, vd, P.tree.pos_scale);
                 if (hit) {  // basis values of this ray -> shared memory, bs[q][lane]
                     float B[BasisCount<KBD>::n];
-                    eval_basis<KBD>(P.tree, P.opt, vd, B);
+                    eval_basis<KBD>(P.tree, opt, vd, B);
 #pragma unroll
                     for (int q = 0; q < KQ; ++q) {
                         float v[4];
@@ -402,7 +410,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) march_queue_kernel(const _
         uint32_t mine_cur = 0u, mine_next = 0u;   // slots of the draining / the following window that hold this lane's samples
         uint32_t qhead = 0u, qcount = 0u;         // warp-uniform
 
-        const bool want_colour = !P.opt.render_depth;
+        const bool want_colour = !opt.render_depth;
 #ifdef VR_POOL_DEBUG
         uint32_t dbg_iter = 0u, dbg_flushes = 0u;
 #endif
@@ -434,7 +442,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) march_queue_kernel(const _
                     if (!want_colour) r = __fmaf_rn(t, weight, r);  // :122-123
                     shaded = want_colour;
                     T = __fmul_rn(T, att);  // :174
-                    stop = T < P.opt.stop_thresh;   // :176
+                    stop = T < opt.stop_thresh;   // :176
                 }
                 t = stop ? __int_as_float(0x7f800000) : __fadd_rn(t, dt);        // :187, or the early-stop marker
             }
@@ -603,23 +611,24 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) march_queue_kernel(const _
         hit = __float_as_uint(t) != 0x7fc00000u;   // lanes without a ray kept the plain NaN
         const bool write_px = packed != 0xffffffffu && lx < P.w && ly < P.h && __float_as_uint(t) != 0x7fc00001u;
         if (write_px) {
+            if constexpr (OUT == kOutViewOpts) vopt = P.opts[view];
             const int px = P.x0 + lx, py = P.y0 + frame_row(P, ly);
             float out[4] = {0.f, 0.f, 0.f, 0.f};
             if (hit) {
-                if (P.opt.render_depth) r = g = b = fminf(r * 0.3f, 1.0f);  // :177-179,189-191
+                if (opt.render_depth) r = g = b = fminf(r * 0.3f, 1.0f);  // :177-179,189-191
                 if (stopped) {  // :181-184
                     const float sc = __frcp_rn(__fsub_rn(1.f, T));
                     out[0] = __fmul_rn(r, sc); out[1] = __fmul_rn(g, sc); out[2] = __fmul_rn(b, sc); out[3] = 1.f;
                 } else {
                     out[0] = r; out[1] = g; out[2] = b;
-                    out[3] = P.opt.render_depth ? 1.f : __fsub_rn(1.f, T);
+                    out[3] = opt.render_depth ? 1.f : __fsub_rn(1.f, T);
                 }
-            } else if (P.tree.N > 0 && P.opt.render_depth) {
+            } else if (P.tree.N > 0 && opt.render_depth) {
                 out[3] = 1.f;  // rt_core.cuh:90-91
             }
             const float nalpha = __fsub_rn(1.f, out[3]);
             if (!P.composite) {
-                const float remain = __fmul_rn(nalpha, P.opt.background_brightness);
+                const float remain = __fmul_rn(nalpha, opt.background_brightness);
                 out[0] = __fadd_rn(remain, out[0]); out[1] = __fadd_rn(remain, out[1]); out[2] = __fadd_rn(remain, out[2]);
             } else {
                 out[0] += (float)(init & 0xffu) / 255.f * nalpha;

@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "volrend_b200.h"
+#include "vr_frames.h"
 
 namespace {
 
@@ -88,8 +89,13 @@ int vr_write_png(const char* path, const uint8_t* rgba8_host, int width, int hei
     return ok ? VR_OK : VR_EINVAL;
 }
 
-int vr_render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
-                         const char* const* paths, int n_threads) {
+}  // extern "C"
+
+namespace {
+
+// vr_render_frames_png(_opts): opt_stride as in vr_frames.h
+int render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
+                      const char* const* paths, int n_threads) {
     if (n_views < 0 || (n_views > 0 && (!cams || !paths))) return VR_EINVAL;
     if (n_views == 0) return VR_OK;
     if (n_threads < 1) n_threads = 1;
@@ -121,7 +127,7 @@ int vr_render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views
     for (int v0 = 0; v0 < n_views; v0 += slab, ++k) {
         const int nv = n_views - v0 < slab ? n_views - v0 : slab;
         uint8_t* dst = buf[k & 1].data();
-        const int rc = vr_render_frames_host(tree, cams + v0, nv, opt, dst);
+        const int rc = vrb::render_frames_host(tree, cams + v0, nv, opt + (size_t)opt_stride * v0, opt_stride, dst);
         if (rc != VR_OK) { if (pending.joinable()) pending.join(); return rc; }
         if (pending.joinable()) pending.join();   // previous slab's buffer is free again after this
         pending = std::thread(encode_slab, dst, v0, nv);
@@ -130,6 +136,20 @@ int vr_render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views
     }
     if (pending.joinable()) pending.join();
     return failed.load() ? VR_EINVAL : VR_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vr_render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
+                         const char* const* paths, int n_threads) {
+    return render_frames_png(tree, cams, n_views, opt, 0, paths, n_threads);
+}
+
+int vr_render_frames_png_opts(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opts,
+                              const char* const* paths, int n_threads) {
+    return render_frames_png(tree, cams, n_views, opts, 1, paths, n_threads);
 }
 
 }  // extern "C"

@@ -128,6 +128,9 @@ struct LaunchDev {
     int32_t blk_mode, blocks_x, n_blocks;
     unsigned char* pool;                // ray-pool kernels: parked-ray stacks, one per CTA (vr_march_q.cuh); nullptr = no parking
     unsigned long long* trace;          // diagnostics: per work item {start ns, end ns, smid, warp}
+    // per-view options (vr_render_batch_opts): device array of n_views entries, read only by the kOutViewOpts
+    // instantiations; nullptr = every view uses `opt`.  Last field, so the other fields keep their offsets.
+    const OptDev* opts;
 };
 
 }  // namespace vrb

@@ -593,18 +593,54 @@ class MultiGpuRenderer:
             pass
 
 
-def render_batch(tree: N3Tree, cams, options: RenderOptions, images, *, float_out=None, counters=None,
+def _per_view(cams, options) -> bool:
+    """True when ``options`` is a sequence of one RenderOptions per camera, False for one RenderOptions."""
+    if isinstance(options, RenderOptions):
+        return False
+    if len(options) != len(cams) or not all(isinstance(o, RenderOptions) for o in options):
+        raise ValueError(f"options: one RenderOptions, or a sequence of {len(cams)} (one per camera)")
+    return True
+
+
+def _options_array(options) -> "C.Array":
+    arr = (_capi.vr_options * len(options))()
+    for i, o in enumerate(options):
+        arr[i] = o._as_c()
+    return arr
+
+
+def render_batch(tree: N3Tree, cams, options, images, *, float_out=None, counters=None,
                  tile=None, stream=None) -> None:
-    """The pose loop of main_headless.cpp:208-223 as one call; ``images``: uint8 [V,H,W,4]."""
+    """The pose loop of main_headless.cpp:208-223 as one call; ``images``: uint8 [V,H,W,4].  ``options`` is one
+    RenderOptions for every view, or a sequence of ``len(cams)`` of them: view i is then rendered with options[i]
+    (vr_render_batch_opts), and ``enable_probe`` draws each view's disc with that view's probe settings."""
     arr = _cams_array(cams)
-    o = options._as_c()
     img = images.data_ptr() if images is not None else None
     fo = float_out.data_ptr() if float_out is not None else None
     s = _stream_ptr(stream)
-    check(lib().vr_render_batch(tree._handle, arr, len(cams), C.byref(o), _rect(tile), img, fo,
-                                counters.data_ptr() if counters is not None else None, s))
-    if options.enable_probe and len(cams):
-        _draw_probe(tree, arr, len(cams), options, o, tile, img, fo, s)
+    cn = counters.data_ptr() if counters is not None else None
+    if not _per_view(cams, options):
+        o = options._as_c()
+        check(lib().vr_render_batch(tree._handle, arr, len(cams), C.byref(o), _rect(tile), img, fo, cn, s))
+        if options.enable_probe and len(cams):
+            _draw_probe(tree, arr, len(cams), options, o, tile, img, fo, s)
+        return
+    oarr = _options_array(options)
+    check(lib().vr_render_batch_opts(tree._handle, arr, len(cams), oarr, _rect(tile), img, fo, cn, s))
+    # the probe disc: one vr_draw_probe per run of consecutive views with the same probe settings
+    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if len(cams) else (0, 0)
+    key = lambda o: (tuple(float(v) for v in o.probe), int(o.probe_disp_size), tuple(int(v) for v in o.basis_minmax))
+    v0 = 0
+    while v0 < len(cams):
+        v1 = v0 + 1
+        if options[v0].enable_probe:
+            while v1 < len(cams) and options[v1].enable_probe and key(options[v1]) == key(options[v0]):
+                v1 += 1
+            sub = (_capi.vr_camera * (v1 - v0)).from_buffer(arr, v0 * C.sizeof(_capi.vr_camera))
+            _draw_probe(tree, sub, v1 - v0, options[v0], oarr[v0], tile,
+                        img + 4 * w * h * v0 if img is not None else None,
+                        fo + 16 * w * h * v0 if fo is not None else None, s)
+        v0 = v1
 
 
 def render_frames_host(tree: N3Tree, cams, options: RenderOptions, host_images) -> None:
@@ -625,11 +661,15 @@ def write_png_file(filename: str, rgba8, width: int | None = None, height: int |
     return lib().vr_write_png(filename.encode(), arr.ctypes.data, int(w), int(h)) == 0
 
 
-def render_frames_png(tree: N3Tree, cams, options: RenderOptions, paths, n_threads: int = 8) -> None:
-    """main_headless.cpp:208-223 with ``-o``: render every pose and write one PNG per pose."""
+def render_frames_png(tree: N3Tree, cams, options, paths, n_threads: int = 8) -> None:
+    """main_headless.cpp:208-223 with ``-o``: render every pose and write one PNG per pose.  ``options``: one
+    RenderOptions, or a sequence of ``len(cams)`` of them (view i rendered with options[i], as render_batch)."""
     arr = _cams_array(cams)
-    o = options._as_c()
     cp = (C.c_char_p * len(paths))(*[p.encode() for p in paths])
+    if _per_view(cams, options):
+        check(lib().vr_render_frames_png_opts(tree._handle, arr, len(cams), _options_array(options), cp, int(n_threads)))
+        return
+    o = options._as_c()
     check(lib().vr_render_frames_png(tree._handle, arr, len(cams), C.byref(o), cp, int(n_threads)))
 
 
