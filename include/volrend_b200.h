@@ -157,6 +157,17 @@ int vr_render_batch_opts(const vr_tree* tree, const vr_camera* cams, int n_views
 int vr_render_composite(const vr_tree* tree, const vr_camera* cam, const vr_options* opt,
                         const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev,
                         float* rgba32f_dev, void* stream);
+/* vr_render_composite for n_views views: view i's colour, depth limit and float output are the i-th tile-sized
+ * frames of rgba8_dev, depth_dev and rgba32f_dev, and its bytes equal vr_render_composite of cams[i].  Tile, the
+ * one-image-size rule and the splitting of very large batches are those of vr_render_batch; _opts renders view i
+ * with opts[i].  Batches of two or more views run on the inline-shading (3 + 16*193) or shading-queue (7) kernel;
+ * any other vr_set_variant setting is VR_EUNSUPPORTED. */
+int vr_render_composite_batch(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
+                              const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev, float* rgba32f_dev,
+                              void* stream);
+int vr_render_composite_batch_opts(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opts,
+                                   const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev,
+                                   float* rgba32f_dev, void* stream);
 
 /* Same, writing a CUDA surface object over an RGBA8 cudaArray (what the reference's
  * caller owns, main_headless.cpp:190-199); depth_surf = 0 => offscreen. */
@@ -313,6 +324,18 @@ typedef struct {
  * length(camera-space position), ready for vr_render_composite.  depth_dev must be >= 0 (1e9 = empty). */
 int vr_draw_meshes(const vr_camera* cam, const vr_mesh_desc* meshes, int n_meshes,
                    uint8_t* rgba8_dev, float* depth_dev, void* stream);
+/* n_views frames of one size (every cams[i] has the same width and height), stored one after another in rgba8_dev
+ * (4*W*H bytes each) and depth_dev (W*H floats each).  View i draws meshes[mesh_off[i] .. mesh_off[i+1]) in that
+ * order.  Its bytes equal
+ *   vr_draw_meshes(&cams[i], meshes + mesh_off[i], mesh_off[i+1] - mesh_off[i], rgba8_dev + i*4*W*H, depth_dev + i*W*H)
+ * exactly (colour and depth).  mesh_off has n_views + 1 entries, non-decreasing, starting at 0.  n_views == 0 and
+ * views without primitives write nothing.  The views with primitives are drawn in launch groups of four launches
+ * each: a group's scratch (8 B of z-buffer per pixel, 16 B per possible large sub-primitive, i.e. 6 per triangle and
+ * 1 per line or point) stays within 256 MiB, unless a single view needs more by itself, and its primitives below
+ * 2^29.  Each view is validated as vr_draw_meshes validates its camera and meshes; views of different sizes, a
+ * NULL, decreasing or non-zero-based mesh_off and a negative n_views are VR_EINVAL. */
+int vr_draw_meshes_batch(const vr_camera* cams, int n_views, const vr_mesh_desc* meshes, const int32_t* mesh_off,
+                         uint8_t* rgba8_dev, float* depth_dev, void* stream);
 
 /* ---- octree grid (volrend_b200/csrc/vr_wire.cu) -----------------------------------------------------------
  * N3Tree::gen_wireframe (src/n3tree.cpp:365-434) generated from the device tree, byte for byte.  Starting at the

@@ -79,6 +79,10 @@ SYMBOLS = {
                                        C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_render_composite": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.POINTER(vr_options),
                                       C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vr_render_composite_batch": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
+                                            C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vr_render_composite_batch_opts": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
+                                                 C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_render_surface": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.POINTER(vr_options),
                                     C.c_ulonglong, C.c_ulonglong, C.c_void_p]),
     "vr_render_frames_host": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
@@ -127,6 +131,8 @@ SYMBOLS = {
     "vr_version": (C.c_char_p, []),
     "vr_draw_meshes": (C.c_int, [C.POINTER(vr_camera), C.POINTER(vr_mesh_desc), C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p]),
+    "vr_draw_meshes_batch": (C.c_int, [C.POINTER(vr_camera), C.c_int, C.POINTER(vr_mesh_desc), C.POINTER(C.c_int32),
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_tree_wireframe": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
     "vr_mesh_estimate_normals": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "vr_tree_compress": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_void_p,

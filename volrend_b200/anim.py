@@ -5,7 +5,7 @@ its Render button is pressed, writes every frame of the fly-through as ``ani_out
 through a GLFW window and ``glReadPixels``.  Here :func:`animation_frames` restates its frame schedule and
 interpolation (``AnimState::update``, main_anim.cpp:230-335) in float32, and :func:`render_animation` renders the
 frames on the GPU: frames without meshes, probe or grid in one batched call with options per frame
-(:func:`volrend_b200.render_frames_png`), the others through :meth:`VolumeRenderer.render`.
+(:func:`volrend_b200.render_frames_png`), the others in chunks through :meth:`VolumeRenderer.render_batch`.
 
     python -m volrend_b200.anim tree.npz keyframes.json -o ani_out/ [-w 800 -h 800] [--fps 30]
                                 [--draw drawlist.npz] [--world_up 0,0,1] [--gpu N]
@@ -24,6 +24,7 @@ import math
 import os
 import sys
 import warnings
+from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -267,11 +268,31 @@ def animation_frames(keyframes, fps: float = 30.0, world_up=(0.0, 0.0, 1.0), cam
 
 
 # ---------------------------------------------------------------------------- rendering
+# Frames per VolumeRenderer.render_batch call of render_animation: bounds its device output and host copies
+# (4 B per pixel per frame, 82 MB at 800x800), of which two chunks are alive while the PNG writers drain one.
+ANIM_CHUNK = 32
+
+
+def _frame_view(state: AnimKF, rend: VolumeRenderer, meshes):
+    """The camera, options and mesh list VolumeRenderer.render() would use for ``state`` (``to_renderer``), with the
+    meshes as shallow copies of ``meshes`` so that frames share their device buffers."""
+    rend.meshes = [copy.copy(m) for m in meshes]
+    state.to_renderer(rend)
+    return copy.deepcopy(rend.camera), rend.options, rend.meshes
+
+
+def _frame_routes(states, names):
+    """For each frame state, whether it goes through VolumeRenderer.render_batch (a visible mesh, the probe or the
+    grid) rather than the plain per-view batch."""
+    return [bool(names & set(s.mesh_state)) or bool(s.opt.enable_probe) or bool(s.opt.show_grid) for s in states]
+
+
 def render_animation(tree, keyframes, fps: float, out_dir: str, *, width: int, height: int, meshes=(),
                      world_up=(0.0, 0.0, 1.0), n_threads: int = 8) -> list:
     """Write every frame of the animation to ``out_dir/%06d.png`` (main_anim.cpp:1255-1257); returns the paths.
     Frames with no visible mesh, no probe and no grid are rendered together, with one RenderOptions per frame, by
-    :func:`render_frames_png`; the others by :meth:`VolumeRenderer.render` (meshes, probe cube and disc, grid).
+    :func:`render_frames_png`; the others in chunks of ``ANIM_CHUNK`` frames by :meth:`VolumeRenderer.render_batch`
+    (meshes, probe cube and disc, grid), whose PNGs ``n_threads`` writers encode while the next chunk renders.
     Each PNG holds exactly what :meth:`VolumeRenderer.render` gives for that frame's state."""
     if not tree.is_cuda_loaded():
         tree.load_cuda()
@@ -281,23 +302,48 @@ def render_animation(tree, keyframes, fps: float, out_dir: str, *, width: int, h
     rend.resize(width, height)
     rend.camera.v_world_up = _vec(world_up).copy()
     os.makedirs(out_dir, exist_ok=True)
-    names = {m.name for m in rend.meshes}
+    base = list(rend.meshes)
+    names = {m.name for m in base}
+    frames = list(animation_frames(keyframes, fps, world_up, Camera(width, height)))
     plain, full = [], []
-    for i, (state, cam) in enumerate(animation_frames(keyframes, fps, world_up, Camera(width, height))):
+    for i, ((state, cam), is_full) in enumerate(zip(frames, _frame_routes([s for s, _ in frames], names))):
         path = os.path.join(out_dir, "%06d.png" % i)
-        if names & set(state.mesh_state) or state.opt.enable_probe or state.opt.show_grid:
+        if is_full:
             full.append((state, path))
         else:
             plain.append((cam, state.opt, path))
     if plain:
         render_frames_png(tree, [c for c, _, _ in plain], [o for _, o, _ in plain], [p for _, _, p in plain],
                           n_threads=n_threads)
-    for state, path in full:
-        state.to_renderer(rend)
-        img = rend.render()
-        if not write_png_file(path, img.cpu().numpy()):
-            raise OSError(f"could not write {path}")
+    if full:
+        for m in base:                       # upload once: every frame's copies share these buffers
+            if m._vert_dev is None:
+                m.update()
+        _render_full_frames(rend, base, full, n_threads)
+        rend.meshes = base
     return sorted([p for _, _, p in plain] + [p for _, p in full])
+
+
+def _write_png(path: str, img) -> None:
+    if not write_png_file(path, img):
+        raise OSError(f"could not write {path}")
+
+
+def _render_full_frames(rend: VolumeRenderer, meshes, full, n_threads: int) -> None:
+    out, pending = None, []
+    with ThreadPoolExecutor(max(int(n_threads), 1)) as pool:
+        for c0 in range(0, len(full), ANIM_CHUNK):
+            chunk = full[c0:c0 + ANIM_CHUNK]
+            views = [_frame_view(state, rend, meshes) for state, _ in chunk]
+            if out is None or out.shape[0] != len(chunk):
+                out = None
+            out = rend.render_batch([v[0] for v in views], [v[1] for v in views], [v[2] for v in views], out=out)
+            host = out.cpu().numpy()         # synchronises: `out` may be rewritten by the next chunk
+            for f in pending:                # at most two chunks of host frames alive
+                f.result()
+            pending = [pool.submit(_write_png, path, host[k]) for k, (_, path) in enumerate(chunk)]
+        for f in pending:
+            f.result()
 
 
 # ---------------------------------------------------------------------------- keyframe files

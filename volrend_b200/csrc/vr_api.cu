@@ -856,7 +856,8 @@ namespace vrb {
 // vr_render_batch (opt_stride 0: one options struct for every view) and vr_render_batch_opts (opt_stride 1: view i
 // uses opt[i]).  A batch of one view is an ordinary single-view launch with that view's options.
 int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
-                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream_) {
+                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream_,
+                 const float* depth_dev) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
     if (n_views == 0) return VR_OK;
@@ -866,12 +867,14 @@ int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_
     for (int i = 1; i < n_views; ++i)
         if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
             return fail(VR_EINVAL, "all views of a batch must share one image size");
+    if (depth_dev && !rgba8_dev) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
     const bool per_view = opt_stride != 0 && n_views > 1;
-    if (per_view) {
-        // the per-view kernels are instantiated for the two product kernels (inline shading, shading queue) only
+    if ((per_view || depth_dev) && n_views > 1) {
+        // per-view options and composite batches are checked on the two product kernels (inline shading, shading
+        // queue) only
         const int v = vr_get_variant();
         if (v != 0 && v != kVariantQueue && v != kVariantInline)
-            return fail(VR_EUNSUPPORTED, "kernel variant %d has no per-view options form", v);
+            return fail(VR_EUNSUPPORTED, "kernel variant %d has no per-view options or composite batch form", v);
     }
     if (r.w == 0 || r.h == 0) return VR_OK;
     LaunchDev P{};
@@ -882,6 +885,7 @@ int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_
     P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
     P.rgba8 = rgba8_dev; P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
     P.counters = counters_dev;
+    P.depth_in = depth_dev; P.composite = depth_dev != nullptr;
     int max_views = kCamRing;  // split very large batches: camera ring size, 31-bit tile index
     if (tile_bound(r) * max_views > 0x7fffffffLL) max_views = (int)(0x7fffffffLL / tile_bound(r));
     if (n_views > max_views) {
@@ -890,7 +894,8 @@ int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_
             const int nv = n_views - v0 < max_views ? n_views - v0 : max_views;
             rc = render_batch(t, cams + v0, nv, opt + (size_t)opt_stride * v0, opt_stride, tile,
                               rgba8_dev ? rgba8_dev + 4 * tile_px * v0 : nullptr,
-                              rgba32f_dev ? rgba32f_dev + 4 * tile_px * v0 : nullptr, counters_dev, stream_);
+                              rgba32f_dev ? rgba32f_dev + 4 * tile_px * v0 : nullptr, counters_dev, stream_,
+                              depth_dev ? depth_dev + tile_px * v0 : nullptr);
             if (rc) return rc;
         }
         return VR_OK;
@@ -912,6 +917,20 @@ int vr_render_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, c
                          const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev,
                          void* stream) {
     return render_batch(t, cams, n_views, opts, 1, tile, rgba8_dev, rgba32f_dev, counters_dev, stream);
+}
+
+int vr_render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
+                              const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev, float* rgba32f_dev,
+                              void* stream) {
+    if (n_views > 0 && (!rgba8_dev || !depth_dev)) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
+    return render_batch(t, cams, n_views, opt, 0, tile, rgba8_dev, rgba32f_dev, nullptr, stream, depth_dev);
+}
+
+int vr_render_composite_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opts,
+                                   const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev,
+                                   float* rgba32f_dev, void* stream) {
+    if (n_views > 0 && (!rgba8_dev || !depth_dev)) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
+    return render_batch(t, cams, n_views, opts, 1, tile, rgba8_dev, rgba32f_dev, nullptr, stream, depth_dev);
 }
 
 int vr_render_bands_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int band_h,
@@ -992,21 +1011,8 @@ int vr_render(const vr_tree* t, const vr_camera* cam, const vr_options* opt, con
 }
 
 int vr_render_composite(const vr_tree* t, const vr_camera* cam, const vr_options* opt, const vr_rect* tile,
-                        uint8_t* rgba8_dev, const float* depth_dev, float* rgba32f_dev, void* stream_) {
-    vr_rect r;
-    int rc = check_common(t, cam, opt, tile, r);
-    if (rc) return rc;
-    if (!rgba8_dev || !depth_dev) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
-    if (r.w == 0 || r.h == 0) return VR_OK;
-    LaunchDev P{};
-    P.tree = t->dev;
-    fill_opt(P.opt, opt);
-    fill_cam(P.cam, cam);
-    P.n_views = 1;
-    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
-    P.rgba8 = rgba8_dev; P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
-    P.depth_in = depth_dev; P.composite = 1;
-    return dispatch(t, P, false, false, (cudaStream_t)stream_);
+                        uint8_t* rgba8_dev, const float* depth_dev, float* rgba32f_dev, void* stream) {
+    return vr_render_composite_batch(t, cam, 1, opt, tile, rgba8_dev, depth_dev, rgba32f_dev, stream);
 }
 
 int vr_render_surface(const vr_tree* t, const vr_camera* cam, const vr_options* opt, unsigned long long rgba8_surf,
@@ -1305,70 +1311,131 @@ int vr_draw_probe(const vr_tree* t, const vr_camera* cams, int n_views, const vr
 // w2c = affineInverse(c2w) (camera.cpp:65), folded with each model matrix in double on the host.
 int vr_draw_meshes(const vr_camera* cam, const vr_mesh_desc* meshes, int n_meshes, uint8_t* rgba8_dev,
                    float* depth_dev, void* stream) {
-    if (!cam) return fail(VR_EINVAL, "null camera");
-    if (cam->width <= 0 || cam->height <= 0) return fail(VR_EINVAL, "zero-size frame %dx%d", cam->width, cam->height);
-    if (cam->width > kRasterMaxSide || cam->height > kRasterMaxSide)
-        return fail(VR_EINVAL, "frame %dx%d exceeds %d pixels per side", cam->width, cam->height, kRasterMaxSide);
     if (n_meshes < 0) return fail(VR_EINVAL, "negative mesh count %d", n_meshes);
-    if (n_meshes > 0 && !meshes) return fail(VR_EINVAL, "null mesh array");
+    const int32_t off[2] = {0, n_meshes};
+    return vr_draw_meshes_batch(cam, 1, meshes, off, rgba8_dev, depth_dev, stream);
+}
+
+// The views are drawn in launch groups: consecutive views with primitives, as many as keep the group's scratch
+// within kRasterScratchBytes, its primitives below kRasterMaxPrims and its views within kRasterMaxViews.
+int vr_draw_meshes_batch(const vr_camera* cams, int n_views, const vr_mesh_desc* meshes, const int32_t* mesh_off,
+                         uint8_t* rgba8_dev, float* depth_dev, void* stream) {
+    if (n_views < 0) return fail(VR_EINVAL, "negative view count %d", n_views);
+    if (n_views == 0) return VR_OK;
+    if (!cams) return fail(VR_EINVAL, "null camera");
+    if (!mesh_off) return fail(VR_EINVAL, "null mesh_off");
+    if (mesh_off[0] != 0) return fail(VR_EINVAL, "mesh_off[0] = %d, not 0", mesh_off[0]);
+    for (int v = 0; v < n_views; ++v)
+        if (mesh_off[v + 1] < mesh_off[v])
+            return fail(VR_EINVAL, "mesh_off decreases at view %d (%d < %d)", v, mesh_off[v + 1], mesh_off[v]);
+    if (mesh_off[n_views] > 0 && !meshes) return fail(VR_EINVAL, "null mesh array");
     if (!rgba8_dev || !depth_dev) return fail(VR_EINVAL, "mesh drawing needs colour and depth buffers");
-    const float* c = cam->c2w;  // column-major 3x4: R[r][k] = c[3k + r], translation c[9..11]
-    double R[3][3], inv[3][3];
-    for (int r = 0; r < 3; ++r)
-        for (int k = 0; k < 3; ++k) R[r][k] = c[3 * k + r];
-    const double det = R[0][0] * (R[1][1] * R[2][2] - R[1][2] * R[2][1]) + R[0][1] * (R[1][2] * R[2][0] - R[1][0] * R[2][2]) +
-                       R[0][2] * (R[1][0] * R[2][1] - R[1][1] * R[2][0]);
-    if (!(det != 0.0) || !std::isfinite(det)) return fail(VR_EINVAL, "camera rotation is singular");
-    inv[0][0] = (R[1][1] * R[2][2] - R[1][2] * R[2][1]) / det;
-    inv[0][1] = (R[0][2] * R[2][1] - R[0][1] * R[2][2]) / det;
-    inv[0][2] = (R[0][1] * R[1][2] - R[0][2] * R[1][1]) / det;
-    inv[1][0] = (R[1][2] * R[2][0] - R[1][0] * R[2][2]) / det;
-    inv[1][1] = (R[0][0] * R[2][2] - R[0][2] * R[2][0]) / det;
-    inv[1][2] = (R[0][2] * R[1][0] - R[0][0] * R[1][2]) / det;
-    inv[2][0] = (R[1][0] * R[2][1] - R[1][1] * R[2][0]) / det;
-    inv[2][1] = (R[0][1] * R[2][0] - R[0][0] * R[2][1]) / det;
-    inv[2][2] = (R[0][0] * R[1][1] - R[0][1] * R[1][0]) / det;
-    double V[3][4];  // w2c rows
-    for (int r = 0; r < 3; ++r) {
-        for (int k = 0; k < 3; ++k) V[r][k] = inv[r][k];
-        V[r][3] = -((inv[r][0] * c[9] + inv[r][1] * c[10]) + inv[r][2] * c[11]);
-    }
+    const int W = cams[0].width, H = cams[0].height;
+    if (W <= 0 || H <= 0) return fail(VR_EINVAL, "zero-size frame %dx%d", W, H);
+    if (W > kRasterMaxSide || H > kRasterMaxSide)
+        return fail(VR_EINVAL, "frame %dx%d exceeds %d pixels per side", W, H, kRasterMaxSide);
+    for (int v = 1; v < n_views; ++v)
+        if (cams[v].width != W || cams[v].height != H)
+            return fail(VR_EINVAL, "view %d is %dx%d, view 0 %dx%d: all views of a batch must share one image size",
+                        v, cams[v].width, cams[v].height, W, H);
+    const long long npx = (long long)W * H;
     std::vector<RasterMesh> rm;
-    long long total = 0, large_cap = 0;
-    for (int i = 0; i < n_meshes; ++i) {
-        const vr_mesh_desc& d = meshes[i];
-        if (d.face_size < 1 || d.face_size > 3)
-            return fail(VR_EINVAL, "mesh %d: face_size %d (1 = points, 2 = lines, 3 = triangles)", i, d.face_size);
-        if (d.n_verts < 0 || d.n_faces < 0)
-            return fail(VR_EINVAL, "mesh %d: negative count (n_verts %d, n_faces %d)", i, d.n_verts, d.n_faces);
-        if (!d.vert_dev && d.n_verts > 0) return fail(VR_EINVAL, "mesh %d: null vert_dev with %d vertices", i, d.n_verts);
-        const long long np = d.faces_dev ? d.n_faces : d.n_verts / d.face_size;
-        if (np == 0) continue;
-        RasterMesh m{};
-        m.vert = d.vert_dev; m.faces = d.faces_dev;
-        m.n_verts = d.n_verts; m.face_size = d.face_size; m.unlit = d.unlit != 0;
-        const float* M = d.model;  // column-major 4x4: M[r][k] = model[4k + r]
-        for (int k = 0; k < 4; ++k)
-            for (int r = 0; r < 3; ++r)
-                m.mv[3 * k + r] = (float)(((V[r][0] * M[4 * k] + V[r][1] * M[4 * k + 1]) + V[r][2] * M[4 * k + 2]) +
-                                          V[r][3] * M[4 * k + 3]);
-        for (int k = 0; k < 3; ++k)
-            for (int r = 0; r < 3; ++r) m.m3[3 * k + r] = M[4 * k + r];
-        m.base = total; m.n_prims = np;
-        total += np;
-        large_cap += np * (d.face_size == 3 ? 6 : 1);
-        if (total >= kRasterMaxPrims) return fail(VR_EINVAL, "more than %lld primitives in one call", kRasterMaxPrims - 1);
-        rm.push_back(m);
+    std::vector<RasterFrame> rf;
+    std::vector<long long> prims, caps;     // per entry of rf
+    std::vector<size_t> first;              // per entry of rf: its first mesh in rm
+    for (int v = 0; v < n_views; ++v) {
+        const vr_camera* cam = &cams[v];
+        const float* c = cam->c2w;  // column-major 3x4: R[r][k] = c[3k + r], translation c[9..11]
+        double R[3][3], inv[3][3];
+        for (int r = 0; r < 3; ++r)
+            for (int k = 0; k < 3; ++k) R[r][k] = c[3 * k + r];
+        const double det = R[0][0] * (R[1][1] * R[2][2] - R[1][2] * R[2][1]) + R[0][1] * (R[1][2] * R[2][0] - R[1][0] * R[2][2]) +
+                           R[0][2] * (R[1][0] * R[2][1] - R[1][1] * R[2][0]);
+        if (!(det != 0.0) || !std::isfinite(det)) return fail(VR_EINVAL, "view %d: camera rotation is singular", v);
+        inv[0][0] = (R[1][1] * R[2][2] - R[1][2] * R[2][1]) / det;
+        inv[0][1] = (R[0][2] * R[2][1] - R[0][1] * R[2][2]) / det;
+        inv[0][2] = (R[0][1] * R[1][2] - R[0][2] * R[1][1]) / det;
+        inv[1][0] = (R[1][2] * R[2][0] - R[1][0] * R[2][2]) / det;
+        inv[1][1] = (R[0][0] * R[2][2] - R[0][2] * R[2][0]) / det;
+        inv[1][2] = (R[0][2] * R[1][0] - R[0][0] * R[1][2]) / det;
+        inv[2][0] = (R[1][0] * R[2][1] - R[1][1] * R[2][0]) / det;
+        inv[2][1] = (R[0][1] * R[2][0] - R[0][0] * R[2][1]) / det;
+        inv[2][2] = (R[0][0] * R[1][1] - R[0][1] * R[1][0]) / det;
+        double V[3][4];  // w2c rows
+        for (int r = 0; r < 3; ++r) {
+            for (int k = 0; k < 3; ++k) V[r][k] = inv[r][k];
+            V[r][3] = -((inv[r][0] * c[9] + inv[r][1] * c[10]) + inv[r][2] * c[11]);
+        }
+        const size_t m0 = rm.size();
+        long long total = 0, large_cap = 0;
+        for (int i = mesh_off[v]; i < mesh_off[v + 1]; ++i) {
+            const vr_mesh_desc& d = meshes[i];
+            if (d.face_size < 1 || d.face_size > 3)
+                return fail(VR_EINVAL, "mesh %d: face_size %d (1 = points, 2 = lines, 3 = triangles)", i, d.face_size);
+            if (d.n_verts < 0 || d.n_faces < 0)
+                return fail(VR_EINVAL, "mesh %d: negative count (n_verts %d, n_faces %d)", i, d.n_verts, d.n_faces);
+            if (!d.vert_dev && d.n_verts > 0) return fail(VR_EINVAL, "mesh %d: null vert_dev with %d vertices", i, d.n_verts);
+            const long long np = d.faces_dev ? d.n_faces : d.n_verts / d.face_size;
+            if (np == 0) continue;
+            RasterMesh m{};
+            m.vert = d.vert_dev; m.faces = d.faces_dev;
+            m.n_verts = d.n_verts; m.face_size = d.face_size; m.unlit = d.unlit != 0;
+            const float* M = d.model;  // column-major 4x4: M[r][k] = model[4k + r]
+            for (int k = 0; k < 4; ++k)
+                for (int r = 0; r < 3; ++r)
+                    m.mv[3 * k + r] = (float)(((V[r][0] * M[4 * k] + V[r][1] * M[4 * k + 1]) + V[r][2] * M[4 * k + 2]) +
+                                              V[r][3] * M[4 * k + 3]);
+            for (int k = 0; k < 3; ++k)
+                for (int r = 0; r < 3; ++r) m.m3[3 * k + r] = M[4 * k + r];
+            m.base = total; m.n_prims = np;     // view-relative here; made launch-wide below
+            total += np;
+            large_cap += np * (d.face_size == 3 ? 6 : 1);
+            if (total >= kRasterMaxPrims)
+                return fail(VR_EINVAL, "view %d: more than %lld primitives", v, kRasterMaxPrims - 1);
+            rm.push_back(m);
+        }
+        if (total == 0) continue;   // nothing to draw: the view's colour and depth stay
+        RasterFrame f{};
+        f.W = W; f.H = H; f.fx = cam->fx; f.fy = cam->fy;
+        f.cx = 0.5f * W; f.cy = 0.5f * H;
+        f.cam_pos[0] = c[9]; f.cam_pos[1] = c[10]; f.cam_pos[2] = c[11];
+        f.rgba8 = rgba8_dev + (size_t)v * 4 * npx;
+        f.depth = depth_dev + (size_t)v * npx;
+        rf.push_back(f);
+        prims.push_back(total);
+        caps.push_back(large_cap);
+        first.push_back(m0);
     }
     int dev = -1;
     if (cudaGetDevice(&dev) != cudaSuccess) return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
-    if (total == 0) return VR_OK;
-    RasterFrame f{};
-    f.W = cam->width; f.H = cam->height; f.fx = cam->fx; f.fy = cam->fy;
-    f.cx = 0.5f * cam->width; f.cy = 0.5f * cam->height;
-    f.cam_pos[0] = c[9]; f.cam_pos[1] = c[10]; f.cam_pos[2] = c[11];
-    VR_CUDA(raster_draw(f, rm.data(), (int)rm.size(), total, large_cap, rgba8_dev, depth_dev, (cudaStream_t)stream));
-    g_launches += kRasterLaunches;
+    first.push_back(rm.size());
+    for (size_t g0 = 0; g0 < rf.size();) {
+        // grow the group while it stays within the bounds; a first view that exceeds kRasterScratchBytes alone
+        // still runs, alone
+        size_t g1 = g0 + 1;
+        long long total = prims[g0];
+        size_t bytes = raster_view_bytes(npx, caps[g0]);
+        while (g1 < rf.size() && g1 - g0 < (size_t)kRasterMaxViews && total + prims[g1] < kRasterMaxPrims &&
+               bytes + raster_view_bytes(npx, caps[g1]) <= kRasterScratchBytes) {
+            total += prims[g1];
+            bytes += raster_view_bytes(npx, caps[g1]);
+            ++g1;
+        }
+        long long base = 0, large_off = 0;
+        for (size_t k = g0; k < g1; ++k) {
+            rf[k].large_off = large_off;
+            large_off += caps[k];
+            for (size_t i = first[k]; i < first[k + 1]; ++i) {
+                rm[i].view = (int)(k - g0);
+                rm[i].base = base;
+                base += rm[i].n_prims;
+            }
+        }
+        VR_CUDA(raster_draw(rf.data() + g0, (int)(g1 - g0), rm.data() + first[g0], (int)(first[g1] - first[g0]), total,
+                            large_off, (cudaStream_t)stream));
+        g_launches += kRasterLaunches;
+        g0 = g1;
+    }
     return VR_OK;
 }
 

@@ -6,8 +6,11 @@
 
 namespace vrb {
 
+// depth_dev != nullptr: composite mode (vr_render_composite_batch): rgba8_dev is read and overwritten, depth_dev
+// holds each view's ray-distance limits, one tile-sized frame per view.
 int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
-                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream);
+                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream,
+                 const float* depth_dev = nullptr);
 
 int render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
                        uint8_t* rgba8_host);

@@ -1,12 +1,13 @@
 // vr_raster.cu -- CUDA rasterizer for VolumeRenderer meshes (the GL mesh pass of cuda_renderer.cpp:83-113,
 // vertex/fragment shaders src/mesh.cpp:98-160, draw :366-396), GL-free.  DESIGN.md section 8.
 //
-// Four launches per call, all on the caller's stream:
+// Four launches per call, all on the caller's stream, each covering every view of the launch (one z-buffer per view;
+// a single-view draw is a launch of one view; DESIGN.md section 15):
 //   z_init      z-buffer key per pixel = (bits(depth_dev), 0)
-//   raster      one thread per primitive: transform, clip, snap; sub-primitives whose pixel bounding box
-//               is at most kSmallPixels are rasterized by that thread, larger ones go to a list
-//   raster_big  one CTA per 32x32 tile of the frame walks that list (a frame-filling triangle is spread
-//               over every CTA instead of one thread)
+//   raster      one thread per primitive of any view: transform, clip, snap; sub-primitives whose pixel bounding
+//               box is at most kSmallPixels are rasterized by that thread, larger ones go to its view's list
+//   raster_big  one CTA per (view, 32x32 tile) walks that view's list (a frame-filling triangle is spread
+//               over every CTA of its view instead of one thread)
 //   resolve     one thread per pixel re-evaluates the primitive that won the pixel: perspective-correct
 //               attributes, the fixed three-light Phong shader, RGBA8 + ray distance
 // Every fragment does one 64-bit atomicMin on (ray-distance bits << 32 | draw sequence number); the
@@ -18,6 +19,8 @@
 #include <stdint.h>
 
 #include <mutex>
+#include <vector>
+#include <string.h>
 
 #include "vr_raster.h"
 
@@ -284,17 +287,22 @@ __device__ __forceinline__ void fragment(const Sub& S, int px, int py, unsigned 
     atomicMin(zbuf + (size_t)py * W + px, frag_key(depth, seq));
 }
 
-__global__ void z_init(const float* __restrict__ depth, unsigned long long* __restrict__ zbuf, long long n) {
+// Grid: (pixel blocks, views).
+__global__ void z_init(const RasterFrame* __restrict__ frames, unsigned long long* __restrict__ zbuf, long long n) {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (i < n) zbuf[i] = frag_key(depth[i], 0u);  // sequence 0: a fragment at the same distance fails (LESS)
+    const float* depth = frames[blockIdx.y].depth;
+    // sequence 0: a fragment at the same distance fails (LESS)
+    if (i < n) zbuf[blockIdx.y * n + i] = frag_key(depth[i], 0u);
 }
 
 __global__ void __launch_bounds__(128) raster(const RasterMesh* __restrict__ meshes, int n_meshes, long long total,
-                                              RasterFrame f, unsigned long long* zbuf, uint4* large,
-                                              unsigned int* n_large) {
+                                              const RasterFrame* __restrict__ frames, unsigned long long* zbuf,
+                                              uint4* large, unsigned int* n_large) {
     const long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (g >= total) return;
     const RasterMesh& m = meshes[find_mesh(meshes, n_meshes, g)];
+    const RasterFrame& f = frames[m.view];
+    zbuf += (size_t)m.view * f.W * f.H;
     Poly P;
     uint32_t idx[3];
     const int nsub = clip_prim(m, g - m.base, f, P, idx);
@@ -303,8 +311,8 @@ __global__ void __launch_bounds__(128) raster(const RasterMesh* __restrict__ mes
         if (!make_sub(m.face_size, P, s, f, S) || S.x0 > S.x1 || S.y0 > S.y1) continue;
         const unsigned int seq = (unsigned int)(g * 8 + s + 1);
         if ((long long)(S.x1 - S.x0 + 1) * (S.y1 - S.y0 + 1) > kSmallPixels) {
-            const unsigned int slot = atomicAdd(n_large, 1u);
-            large[slot] = make_uint4(seq, (unsigned)S.x0 | ((unsigned)S.y0 << 16),
+            const unsigned int slot = atomicAdd(n_large + m.view, 1u);
+            large[f.large_off + slot] = make_uint4(seq, (unsigned)S.x0 | ((unsigned)S.y0 << 16),
                                      (unsigned)S.x1 | ((unsigned)S.y1 << 16), 0u);
             continue;
         }
@@ -325,13 +333,19 @@ __device__ __forceinline__ bool load_sub(const RasterMesh* meshes, int n_meshes,
     return s < nsub && make_sub(m.face_size, P, s, f, S);
 }
 
-__global__ void __launch_bounds__(256) raster_big(const RasterMesh* __restrict__ meshes, int n_meshes, RasterFrame f,
-                                                  unsigned long long* zbuf, const uint4* __restrict__ large,
+// Grid: (tile columns, tile rows, views); a CTA walks its own view's list only.  Three CTAs per SM: without the bound
+// the per-view frame pointer raises the kernel to 100 registers (two CTAs).
+__global__ void __launch_bounds__(256, 3) raster_big(const RasterMesh* __restrict__ meshes, int n_meshes,
+                                                  const RasterFrame* __restrict__ frames, unsigned long long* zbuf,
+                                                  const uint4* __restrict__ large,
                                                   const unsigned int* __restrict__ n_large) {
+    const RasterFrame& f = frames[blockIdx.z];
+    zbuf += (size_t)blockIdx.z * f.W * f.H;
+    large += f.large_off;
     const int tx0 = blockIdx.x * kTile, ty0 = blockIdx.y * kTile;
     const int tx1 = min(tx0 + kTile - 1, f.W - 1), ty1 = min(ty0 + kTile - 1, f.H - 1);
     const int px = tx0 + (threadIdx.x & (kTile - 1));
-    const unsigned int n = *n_large;
+    const unsigned int n = n_large[blockIdx.z];
     for (unsigned int e = 0; e < n; ++e) {
         const uint4 L = large[e];
         const int x0 = L.y & 0xffff, y0 = L.y >> 16, x1 = L.z & 0xffff, y1 = L.z >> 16;
@@ -356,13 +370,15 @@ __device__ __forceinline__ uint8_t to_u8(float v) {
     return (uint8_t)__float2int_rn(fm(fminf(fmaxf(v, 0.f), 1.f), 255.f));
 }
 
-__global__ void __launch_bounds__(128) resolve(const RasterMesh* __restrict__ meshes, int n_meshes, RasterFrame f,
-                                               const unsigned long long* __restrict__ zbuf, uint8_t* rgba8,
-                                               float* depth) {
+// Grid: (32-pixel columns, 4-pixel rows, views).
+__global__ void __launch_bounds__(128) resolve(const RasterMesh* __restrict__ meshes, int n_meshes,
+                                               const RasterFrame* __restrict__ frames,
+                                               const unsigned long long* __restrict__ zbuf) {
+    const RasterFrame& f = frames[blockIdx.z];
     const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 4 + (threadIdx.x >> 5);
     if (x >= f.W || y >= f.H) return;
-    const size_t p = (size_t)y * f.W + x;
-    const unsigned int seq = (unsigned int)zbuf[p];
+    const unsigned int p = (unsigned int)(y * f.W + x);   // W * H <= 2^30
+    const unsigned int seq = (unsigned int)zbuf[(size_t)blockIdx.z * f.W * f.H + p];
     if (seq == 0u) return;  // no fragment beat the incoming depth: colour and depth stay
     Sub S;
     const RasterMesh* mp;
@@ -416,8 +432,8 @@ __global__ void __launch_bounds__(128) resolve(const RasterMesh* __restrict__ me
     }
     uchar4 o;
     o.x = to_u8(out[0]); o.y = to_u8(out[1]); o.z = to_u8(out[2]); o.w = to_u8(out[3]);
-    reinterpret_cast<uchar4*>(rgba8)[p] = o;
-    depth[p] = dist;
+    reinterpret_cast<uchar4*>(f.rgba8)[p] = o;
+    f.depth[p] = dist;
 }
 
 }  // namespace
@@ -448,12 +464,16 @@ cudaError_t scratch_pool(cudaMemPool_t* out) {
     return cudaSuccess;
 }
 
-cudaError_t raster_draw(const RasterFrame& f, const RasterMesh* meshes, int n, long long total_prims,
-                        long long large_cap, uint8_t* rgba8, float* depth, cudaStream_t st) {
-    const long long npx = (long long)f.W * f.H;
-    const size_t z_bytes = (size_t)npx * 8, m_bytes = sizeof(RasterMesh) * (size_t)n;
-    const size_t m_off = z_bytes, c_off = (m_off + m_bytes + 15) / 16 * 16, l_off = c_off + 16;
-    const size_t bytes = l_off + (size_t)large_cap * sizeof(uint4);
+cudaError_t raster_draw(const RasterFrame* frames, int n_views, const RasterMesh* meshes, int n, long long total_prims,
+                        long long large_total, cudaStream_t st) {
+    const int W = frames[0].W, H = frames[0].H;
+    const long long npx = (long long)W * H;
+    // scratch: z-buffers | meshes | frames | per-view list counters | large-primitive lists
+    const size_t z_bytes = (size_t)npx * 8 * n_views, m_bytes = sizeof(RasterMesh) * (size_t)n;
+    const size_t f_bytes = sizeof(RasterFrame) * (size_t)n_views, c_bytes = ((size_t)n_views * 4 + 15) / 16 * 16;
+    const size_t m_off = z_bytes, f_off = (m_off + m_bytes + 15) / 16 * 16, c_off = (f_off + f_bytes + 15) / 16 * 16;
+    const size_t l_off = c_off + c_bytes;
+    const size_t bytes = l_off + (size_t)large_total * sizeof(uint4);
     cudaMemPool_t pool;
     cudaError_t e = scratch_pool(&pool);
     if (e != cudaSuccess) return e;
@@ -461,16 +481,21 @@ cudaError_t raster_draw(const RasterFrame& f, const RasterMesh* meshes, int n, l
     if ((e = cudaMallocFromPoolAsync((void**)&scratch, bytes, pool, st)) != cudaSuccess) return e;
     unsigned long long* zbuf = reinterpret_cast<unsigned long long*>(scratch);
     RasterMesh* dmesh = reinterpret_cast<RasterMesh*>(scratch + m_off);
+    RasterFrame* dframe = reinterpret_cast<RasterFrame*>(scratch + f_off);
     unsigned int* n_large = reinterpret_cast<unsigned int*>(scratch + c_off);
     uint4* large = reinterpret_cast<uint4*>(scratch + l_off);
-    // pageable source: the copy has been staged when cudaMemcpyAsync returns
-    if ((e = cudaMemcpyAsync(dmesh, meshes, m_bytes, cudaMemcpyHostToDevice, st)) == cudaSuccess &&
-        (e = cudaMemsetAsync(n_large, 0, 16, st)) == cudaSuccess) {
-        z_init<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(depth, zbuf, npx);
-        raster<<<(unsigned)((total_prims + 127) / 128), 128, 0, st>>>(dmesh, n, total_prims, f, zbuf, large, n_large);
-        raster_big<<<dim3((f.W + kTile - 1) / kTile, (f.H + kTile - 1) / kTile), 256, 0, st>>>(dmesh, n, f, zbuf,
-                                                                                                large, n_large);
-        resolve<<<dim3((f.W + 31) / 32, (f.H + 3) / 4), 128, 0, st>>>(dmesh, n, f, zbuf, rgba8, depth);
+    // meshes and frames in one copy, counters zeroed behind them; pageable source: the copy has been staged when
+    // cudaMemcpyAsync returns
+    std::vector<unsigned char> h(c_off + c_bytes - m_off, 0);
+    memcpy(h.data(), meshes, m_bytes);
+    memcpy(h.data() + (f_off - m_off), frames, f_bytes);
+    if ((e = cudaMemcpyAsync(dmesh, h.data(), h.size(), cudaMemcpyHostToDevice, st)) == cudaSuccess) {
+        z_init<<<dim3((unsigned)((npx + 255) / 256), n_views), 256, 0, st>>>(dframe, zbuf, npx);
+        raster<<<(unsigned)((total_prims + 127) / 128), 128, 0, st>>>(dmesh, n, total_prims, dframe, zbuf, large,
+                                                                      n_large);
+        raster_big<<<dim3((W + kTile - 1) / kTile, (H + kTile - 1) / kTile, n_views), 256, 0, st>>>(
+            dmesh, n, dframe, zbuf, large, n_large);
+        resolve<<<dim3((W + 31) / 32, (H + 3) / 4, n_views), 128, 0, st>>>(dmesh, n, dframe, zbuf);
         e = cudaGetLastError();
     }
     const cudaError_t e2 = cudaFreeAsync(scratch, st);

@@ -17,6 +17,7 @@ PyTorch is used only to own device memory and streams.  The compiled C++ shim
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import os
 from dataclasses import dataclass, field
@@ -627,14 +628,20 @@ def render_batch(tree: N3Tree, cams, options, images, *, float_out=None, counter
         return
     oarr = _options_array(options)
     check(lib().vr_render_batch_opts(tree._handle, arr, len(cams), oarr, _rect(tile), img, fo, cn, s))
-    # the probe disc: one vr_draw_probe per run of consecutive views with the same probe settings
-    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if len(cams) else (0, 0)
+    _draw_probe_runs(tree, arr, options, oarr, tile, img, fo, s)
+
+
+def _draw_probe_runs(tree: N3Tree, arr, options, oarr, tile, img, fo, s) -> None:
+    """The probe discs of a batch rendered with options per view (``arr`` cameras, ``oarr`` their vr_options): one
+    vr_draw_probe per run of consecutive views with the same probe settings."""
+    n = len(options)
+    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (arr[0].width, arr[0].height) if n else (0, 0)
     key = lambda o: (tuple(float(v) for v in o.probe), int(o.probe_disp_size), tuple(int(v) for v in o.basis_minmax))
     v0 = 0
-    while v0 < len(cams):
+    while v0 < n:
         v1 = v0 + 1
         if options[v0].enable_probe:
-            while v1 < len(cams) and options[v1].enable_probe and key(options[v1]) == key(options[v0]):
+            while v1 < n and options[v1].enable_probe and key(options[v1]) == key(options[v0]):
                 v1 += 1
             sub = (_capi.vr_camera * (v1 - v0)).from_buffer(arr, v0 * C.sizeof(_capi.vr_camera))
             _draw_probe(tree, sub, v1 - v0, options[v0], oarr[v0], tile,
@@ -723,12 +730,14 @@ class VolumeRenderer:
         self._tree = None
         self._wire = self._wire_depth = None
 
-    def _grid_mesh(self):
-        """The grid mesh to draw, or None (cuda_renderer.cpp maybe_gen_wire): regenerated on the device when
-        ``grid_max_depth`` changed since the last one.  Without a loaded tree there is no grid."""
-        if not self.options.show_grid or self._tree is None or not self._tree.is_cuda_loaded():
+    def _grid_mesh(self, options=None):
+        """The grid mesh to draw with ``options`` (default ``self.options``), or None (cuda_renderer.cpp
+        maybe_gen_wire): regenerated on the device when ``grid_max_depth`` changed since the last one.  Without a
+        loaded tree there is no grid."""
+        options = self.options if options is None else options
+        if not options.show_grid or self._tree is None or not self._tree.is_cuda_loaded():
             return None
-        depth = int(self.options.grid_max_depth)
+        depth = int(options.grid_max_depth)
         if self._wire is None or self._wire_depth != depth:
             from .mesh import Mesh
             n = self._tree.wireframe_vertex_count(depth)
@@ -791,3 +800,91 @@ class VolumeRenderer:
             return self._image
         launch_renderer(self._tree, self.camera, self.options, self._image, None, None, True)
         return self._image
+
+    def render_batch(self, cams, options=None, meshes=None, out=None):
+        """Renders ``len(cams)`` views and returns them as a CUDA uint8 tensor [V,H,W,4] (``out`` if given).  View i
+        is byte for byte what :meth:`render` returns after ``camera = cams[i]``, ``options = options[i]`` and
+        ``meshes = meshes[i]``: the cleared background, the meshes, probe cube and grid, the composited volume and the
+        probe disc, or the offscreen march for views with none of these.  ``options``: None (``self.options``), one
+        :class:`RenderOptions` or one per view; ``meshes``: None (``self.meshes`` for every view) or one list of
+        :class:`~volrend_b200.Mesh` per view, which may hold shallow copies (``copy.copy(mesh)``) of one uploaded mesh
+        with their own transform, ``visible`` and ``unlit``.  Every camera has the same size; the cameras are not
+        modified.  Views are rendered in runs of consecutive views of one kind, a mesh run in one batched draw and
+        one batched composite march per chunk of at most ``RENDER_BATCH_CHUNK`` views."""
+        import torch
+        from .mesh import draw_meshes_batch
+        if self._image is None:
+            raise RuntimeError("VolumeRenderer needs a CUDA device (no CPU fallback)")
+        n = len(cams)
+        if options is None:
+            options = self.options
+        opts = [options] * n if isinstance(options, RenderOptions) else list(options)
+        _per_view(cams, opts)
+        mlists = [self.meshes] * n if meshes is None else list(meshes)
+        if len(mlists) != n:
+            raise ValueError(f"meshes: None or a sequence of {n} mesh lists (one per camera)")
+        cams = [copy.deepcopy(c) for c in cams]
+        for c in cams:
+            c._update()
+        if n and any((c.width, c.height) != (cams[0].width, cams[0].height) for c in cams):
+            raise ValueError("render_batch: every camera must have the same size")
+        h, w = (cams[0].height, cams[0].width) if n else (0, 0)
+        if out is None:
+            out = torch.empty((n, h, w, 4), dtype=torch.uint8, device=self._image.device)
+        elif tuple(out.shape) != (n, h, w, 4) or out.dtype != torch.uint8 or not out.is_cuda or not out.is_contiguous():
+            raise ValueError(f"out: expected a contiguous CUDA uint8 tensor of shape {(n, h, w, 4)}")
+        tree = self._tree if self._tree is not None and self._tree.is_cuda_loaded() else None
+        draws, wires = [], {}
+        for o, ms in zip(opts, mlists):
+            vis = [m for m in ms if m.visible]
+            if o.enable_probe:                       # render(): the probe cube at options.probe
+                p = copy.copy(self._probe)
+                p.visible = True
+                p.translation = np.asarray(o.probe, np.float32).reshape(3).copy()
+                vis.append(p)
+            if o.show_grid and tree is not None:     # one grid per distinct depth in the call
+                d = int(o.grid_max_depth)
+                if d not in wires:
+                    wires[d] = self._grid_mesh(o)
+                vis.append(wires[d])
+            draws.append(vis)
+        s = _stream_ptr(None)
+        for mesh_run, v0, v1 in _view_runs([bool(d) for d in draws], RENDER_BATCH_CHUNK):
+            img, run_cams, run_opts = out[v0:v1], cams[v0:v1], opts[v0:v1]
+            bg = [float(o.background_brightness) for o in run_opts]
+            if mesh_run:
+                dep = torch.full((v1 - v0, h, w), 1e9, dtype=torch.float32, device=out.device)
+                bgv = torch.tensor([round(min(max(b, 0.0), 1.0) * 255) for b in bg], dtype=torch.uint8)
+                img[..., :3] = bgv.to(out.device, non_blocking=True).view(-1, 1, 1, 1)
+                img[..., 3] = 255
+                draw_meshes_batch(run_cams, draws[v0:v1], img, dep)
+                if tree is not None:
+                    arr, oarr = _cams_array(run_cams), _options_array(run_opts)
+                    check(lib().vr_render_composite_batch_opts(tree._handle, arr, v1 - v0, oarr, None, img.data_ptr(),
+                                                               dep.data_ptr(), None, s))
+                    _draw_probe_runs(tree, arr, run_opts, oarr, None, img.data_ptr(), None, s)
+            elif tree is not None:
+                render_batch(tree, run_cams, run_opts, img)
+            else:                                    # render() without a tree: int(bg * 255), no clamp
+                bgv = torch.tensor([int(b * 255) & 0xFF for b in bg], dtype=torch.uint8)
+                img[..., :3] = bgv.to(out.device, non_blocking=True).view(-1, 1, 1, 1)
+                img[..., 3] = 255
+        return out
+
+
+# Views per batched draw and composite march in VolumeRenderer.render_batch: bounds the ray-distance buffer it
+# allocates (4 B per pixel per view, 82 MB at 800x800).
+RENDER_BATCH_CHUNK = 32
+
+
+def _view_runs(has_draw, chunk: int):
+    """Splits views into runs of consecutive views of one kind (True: something to draw before the march), each at
+    most ``chunk`` long: a list of (kind, v0, v1) in view order."""
+    runs, v0 = [], 0
+    while v0 < len(has_draw):
+        v1 = v0 + 1
+        while v1 < len(has_draw) and v1 - v0 < chunk and has_draw[v1] == has_draw[v0]:
+            v1 += 1
+        runs.append((bool(has_draw[v0]), v0, v1))
+        v0 = v1
+    return runs

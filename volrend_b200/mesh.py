@@ -333,6 +333,36 @@ def estimate_normals(mesh: Mesh, stream=None) -> None:
     mesh.vert = vd.cpu().numpy()
 
 
+def _mesh_table(meshes_per_view):
+    """The descriptors of every view's visible meshes, view after view, and the ``mesh_off`` offsets (n_views + 1
+    entries) that delimit each view's run of them."""
+    per_view = [[m for m in ms if m.visible] for ms in meshes_per_view]
+    off = np.zeros(len(per_view) + 1, np.int32)
+    off[1:] = np.cumsum([len(v) for v in per_view], dtype=np.int64)
+    arr = (_capi.vr_mesh_desc * max(int(off[-1]), 1))()
+    i = 0
+    for vis in per_view:
+        for m in vis:
+            arr[i] = m._as_c()
+            i += 1
+    return arr, (C.c_int32 * len(off))(*[int(v) for v in off])
+
+
+def draw_meshes_batch(cams, meshes_per_view, images, depth, stream=None) -> None:
+    """:func:`draw_meshes` for many views in one call (``vr_draw_meshes_batch``): view i draws the visible meshes of
+    ``meshes_per_view[i]`` with ``cams[i]`` over ``images[i]`` (CUDA uint8 [V,H,W,4]) and ``depth[i]`` (CUDA float32
+    [V,H,W]), byte for byte what :func:`draw_meshes` would draw.  Every camera has the same size.  A list may hold
+    shallow copies (``copy.copy(mesh)``) of one uploaded mesh with their own transform, ``visible`` and ``unlit``:
+    they share its device buffers, so nothing is uploaded per view."""
+    from .host import _cams_array, _stream_ptr
+    if len(meshes_per_view) != len(cams):
+        raise ValueError(f"meshes_per_view: expected {len(cams)} lists (one per camera), got {len(meshes_per_view)}")
+    arr, off = _mesh_table(meshes_per_view)
+    check(lib().vr_draw_meshes_batch(_cams_array(cams), len(cams), arr, off,
+                                     images.data_ptr() if images is not None else None,
+                                     depth.data_ptr() if depth is not None else None, _stream_ptr(stream)))
+
+
 def draw_meshes(cam, meshes, image, depth, stream=None) -> None:
     """Draws the visible ``meshes`` in order over ``image`` (CUDA uint8 [H,W,4]) and ``depth`` (CUDA float32
     [H,W], ray distance; GL depth test LESS against it).  Covered pixels receive the mesh colour and the
