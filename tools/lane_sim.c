@@ -17,6 +17,7 @@
 typedef struct {
     uint32_t off;   /* first sample in the trace */
     uint32_t n;     /* samples */
+    uint32_t koff;  /* MEM mode: first key in g_keys */
     uint8_t hit;
 } ray_t;
 
@@ -25,6 +26,11 @@ static const int g_p3_theta[6] = {4, 8, 12, 8, 8, 4}, g_p3_pat[6] = {1, 1, 1, 8,
 static int g_b[32];   /* cumulative levels resolved after table k */
 static uint8_t* g_trace;  /* per sample: fetches (low 4 bits) | shaded << 7 */
 static size_t g_trace_n, g_trace_cap;
+/* MEM mode: per sample its `fetches` table-word sector keys, then (if shaded) its record key; ray_t::off indexes both
+   streams' first sample / key through g_koff */
+static uint32_t* g_keys;
+static size_t g_keys_n, g_keys_cap;
+static int g_mem;
 
 static void push(uint8_t v) {
     if (g_trace_n == g_trace_cap) {
@@ -34,10 +40,19 @@ static void push(uint8_t v) {
     g_trace[g_trace_n++] = v;
 }
 
+static void push_key(uint64_t k) {
+    if (k >= (1ull << 32)) { fprintf(stderr, "key overflow\n"); exit(1); }
+    if (g_keys_n == g_keys_cap) {
+        g_keys_cap = g_keys_cap ? g_keys_cap * 2 : (1u << 24);
+        g_keys = (uint32_t*)realloc(g_keys, g_keys_cap * 4);
+    }
+    g_keys[g_keys_n++] = (uint32_t)k;
+}
+
 /* the march of trace_ray() above without colours; records wide-table fetch counts */
 static void trace_one(const orc_tree* tree, const orc_camera* cam, const orc_options* opt, int x, int y, ray_t* R) {
     float dir[3], cen[3];
-    R->off = (uint32_t)g_trace_n; R->n = 0; R->hit = 0;
+    R->off = (uint32_t)g_trace_n; R->n = 0; R->hit = 0; R->koff = (uint32_t)g_keys_n;
     screen2worlddir(x, y, cam, dir, cen);
     maybe_world2ndc(tree, dir, cen);
     for (int i = 0; i < 3; ++i) cen[i] = fmaf(tree->scale[i], cen[i], tree->offset[i]);
@@ -74,7 +89,9 @@ static void trace_one(const orc_tree* tree, const orc_camera* cam, const orc_opt
         int64_t ptr = 0, sub;
         float cube = 2.f;
         int depth = 0;
+        int64_t node_at[32];   /* node id at each depth of the path (its children start at child[8 * id]) */
         for (;;) {
+            node_at[depth] = ptr >> 3;
             float index = 0.f;
             for (int i = 0; i < 3; ++i) {
                 pos[i] = pos[i] * 2.f;
@@ -99,6 +116,16 @@ static void trace_one(const orc_tree* tree, const orc_camera* cam, const orc_opt
         while (g_b[jl] < depth) ++jl;
         int fetches = jl - j0 + 1;
         if (fetches < 1) fetches = 1;
+        if (j0 > jl) j0 = jl;
+        uint64_t entry = 0;
+        for (int k = j0; g_mem && k <= jl; ++k) {
+            /* table k hangs off the path's node of depth g_b[k-1] and is indexed by the x | y | z bits of its levels
+               (vr_march.cuh find_leaf_wide); a table is 64 words = 8 sectors, so only the 32-byte sector matters */
+            const int rd = k ? g_b[k - 1] : 0, lv = g_b[k] - rd, sh = 24 - g_b[k];
+            const uint32_t m = (1u << lv) - 1;
+            entry = (uint64_t)node_at[rd] * 64 + ((((u[0] >> sh) & m) << (2 * lv)) | (((u[1] >> sh) & m) << lv) | ((u[2] >> sh) & m));
+            push_key(entry >> 3);
+        }
         pu[0] = u[0]; pu[1] = u[1]; pu[2] = u[2]; pdepth = depth;
         float tsub = 1e4f;
         for (int i = 0; i < 3; ++i) {
@@ -116,6 +143,7 @@ static void trace_one(const orc_tree* tree, const orc_camera* cam, const orc_opt
             if (light < opt->stop_thresh) stop = 1;
         }
         push((uint8_t)(fetches | (shaded << 7)));
+        if (g_mem && shaded) push_key(entry);   /* records are indexed by the leaf's table entry */
         R->n++;
         if (stop) break;
         t += dt;
@@ -317,6 +345,202 @@ static void sim_park(const ray_t* rays, int W, int H, int theta, int patience, s
     }
 }
 
+/* ---- MEM mode: DRAM traffic of a work order.  The tiles of all views are handed out in queue order to NW warps (a
+ * warp takes the next tile when its current one ends); all busy warps advance one march iteration per round, and every
+ * table-word fetch (a 32-byte sector of its table) and every shaded sample's 96-byte record (3 sectors, keyed by its
+ * table entry) goes through an LRU model of the L2 in 32-byte sectors.  No associativity, no L1, no cache hints. */
+typedef struct {
+    uint64_t* key;    /* hash table: key + 1 (0 = empty), linear probing */
+    int32_t* slot;
+    uint64_t* skey;   /* LRU list over slots */
+    int32_t *prev, *next;
+    uint64_t mask;
+    int32_t cap, n, head, tail;
+} lru_t;
+
+static inline uint64_t hmix(uint64_t k) { k *= 0x9E3779B97F4A7C15ull; return k ^ (k >> 29); }
+
+static void lru_init(lru_t* L, int cap) {
+    uint64_t hs = 1;
+    while (hs < (uint64_t)cap * 2) hs <<= 1;
+    L->key = (uint64_t*)calloc(hs, 8); L->slot = (int32_t*)malloc(hs * 4); L->mask = hs - 1;
+    L->skey = (uint64_t*)malloc((size_t)cap * 8);
+    L->prev = (int32_t*)malloc((size_t)cap * 4); L->next = (int32_t*)malloc((size_t)cap * 4);
+    L->cap = cap; L->n = 0; L->head = L->tail = -1;
+}
+static void lru_free(lru_t* L) { free(L->key); free(L->slot); free(L->skey); free(L->prev); free(L->next); }
+static inline void lru_unlink(lru_t* L, int s) {
+    if (L->prev[s] >= 0) L->next[L->prev[s]] = L->next[s]; else L->head = L->next[s];
+    if (L->next[s] >= 0) L->prev[L->next[s]] = L->prev[s]; else L->tail = L->prev[s];
+}
+static inline void lru_front(lru_t* L, int s) {
+    L->prev[s] = -1; L->next[s] = L->head;
+    if (L->head >= 0) L->prev[L->head] = s;
+    L->head = s;
+    if (L->tail < 0) L->tail = s;
+}
+static void hash_del(lru_t* L, uint64_t k) {   /* backward-shift deletion */
+    uint64_t i = hmix(k) & L->mask;
+    while (L->key[i] != k + 1) i = (i + 1) & L->mask;
+    for (;;) {
+        uint64_t j = i;
+        for (;;) {
+            j = (j + 1) & L->mask;
+            if (!L->key[j]) { L->key[i] = 0; return; }
+            const uint64_t h = hmix(L->key[j] - 1) & L->mask;   /* j's entry may fill i unless its home is in (i, j] */
+            if (i <= j ? (h <= i || h > j) : (h <= i && h > j)) break;
+        }
+        L->key[i] = L->key[j]; L->slot[i] = L->slot[j];
+        i = j;
+    }
+}
+static inline int lru_touch(lru_t* L, uint64_t k) {   /* 1 on a miss */
+    uint64_t i = hmix(k) & L->mask;
+    while (L->key[i]) {
+        if (L->key[i] == k + 1) {
+            const int s = L->slot[i];
+            if (L->head != s) { lru_unlink(L, s); lru_front(L, s); }
+            return 0;
+        }
+        i = (i + 1) & L->mask;
+    }
+    int s;
+    if (L->n < L->cap) {
+        s = L->n++;
+    } else {
+        s = L->tail;
+        lru_unlink(L, s);
+        hash_del(L, L->skey[s]);
+        i = hmix(k) & L->mask;
+        while (L->key[i]) i = (i + 1) & L->mask;
+    }
+    L->key[i] = k + 1; L->slot[i] = s; L->skey[s] = k;
+    lru_front(L, s);
+    return 1;
+}
+
+typedef struct {
+    const char* name;
+    const ray_t* const* vrays;    /* rays of each view */
+    const int32_t* tiles;         /* (view, tx, ty) per queue item */
+    int ntiles, W, H, nw, cap;
+    double tbl_acc, tbl_miss, rec_acc, rec_miss, rounds;
+} replay_t;
+
+static void* replay(void* arg) {
+    replay_t* J = (replay_t*)arg;
+    const int TW = 4, TH = 8;
+    const uint64_t kRec = 1ull << 40;   /* record sectors: their own address range */
+    lru_t L;
+    lru_init(&L, J->cap);
+    const ray_t** lane = (const ray_t**)calloc((size_t)J->nw * 32, sizeof(ray_t*));
+    uint32_t* pos = (uint32_t*)calloc((size_t)J->nw * 32, 4);
+    uint32_t* kp = (uint32_t*)calloc((size_t)J->nw * 32, 4);
+    int* alive = (int*)calloc(J->nw, sizeof(int));
+    char* busy = (char*)calloc(J->nw, 1);
+    int next = 0;
+    for (;;) {
+        int any = 0;
+        for (int w = 0; w < J->nw; ++w) {
+            const ray_t** ln = lane + (size_t)w * 32;
+            uint32_t* ps = pos + (size_t)w * 32;
+            uint32_t* kq = kp + (size_t)w * 32;
+            if (!busy[w]) {
+                if (next >= J->ntiles) continue;
+                const int32_t* t = J->tiles + 3 * (size_t)next++;
+                const ray_t* rays = J->vrays[t[0]];
+                alive[w] = 0;
+                for (int l = 0; l < 32; ++l) {
+                    const int x = t[1] * TW + l % TW, y = t[2] * TH + l / TW;
+                    ln[l] = (x < J->W && y < J->H) ? &rays[(size_t)y * J->W + x] : NULL;
+                    ps[l] = 0;
+                    if (ln[l]) { kq[l] = ln[l]->koff; if (ln[l]->n) ++alive[w]; }
+                }
+                busy[w] = 1;
+            }
+            any = 1;
+            for (int l = 0; l < 32; ++l) {
+                if (!ln[l] || ps[l] >= ln[l]->n) continue;
+                const uint8_t v = g_trace[ln[l]->off + ps[l]++];
+                for (int f = v & 15; f > 0; --f) { J->tbl_acc += 1; J->tbl_miss += lru_touch(&L, g_keys[kq[l]++]); }
+                if (v & 128) {
+                    const uint64_t r = (uint64_t)g_keys[kq[l]++] * 3;
+                    J->rec_acc += 1;
+                    for (int s = 0; s < 3; ++s) J->rec_miss += lru_touch(&L, kRec + r + s);
+                }
+                if (ps[l] >= ln[l]->n) --alive[w];
+            }
+            if (alive[w] <= 0) busy[w] = 0;
+        }
+        if (!any) break;
+        J->rounds += 1;
+    }
+    free(lane); free(pos); free(kp); free(alive); free(busy);
+    lru_free(&L);
+    return NULL;
+}
+
+static inline int centre_out(int r, int rows) {   /* vr_march.cuh decode_item */
+    const int half = rows >> 1;
+    return r < 2 * half ? ((r & 1) ? half + (r >> 1) : half - 1 - (r >> 1)) : r;
+}
+
+/* group = 0: view-major (all tiles of view 0, then view 1, ...); group = g: tile rows outermost inside each group of
+   g consecutive views, views inside rows, tx innermost (g >= ncam: one group, row-major across the whole launch) */
+static int32_t* make_order(int ncam, int ntx, int nty, int group) {
+    int32_t* t = (int32_t*)malloc((size_t)ncam * ntx * nty * 3 * 4);
+    size_t k = 0;
+    if (!group) {
+        for (int v = 0; v < ncam; ++v)
+            for (int r = 0; r < nty; ++r)
+                for (int x = 0; x < ntx; ++x) { t[k++] = v; t[k++] = x; t[k++] = centre_out(r, nty); }
+        return t;
+    }
+    for (int g0 = 0; g0 < ncam; g0 += group)
+        for (int r = 0; r < nty; ++r)
+            for (int v = g0; v < g0 + group && v < ncam; ++v)
+                for (int x = 0; x < ntx; ++x) { t[k++] = v; t[k++] = x; t[k++] = centre_out(r, nty); }
+    return t;
+}
+
+static void mem_main(const orc_tree* tree, const orc_camera* cams, int ncam, int W, int H) {
+    const int nw = getenv("NWARPS") ? atoi(getenv("NWARPS")) : 4224;   /* 8 CTAs x 4 warps x 132 SMs */
+    const double l2mb = getenv("L2MB") ? atof(getenv("L2MB")) : 50.0;
+    const int cap = (int)(l2mb * 1024 * 1024 / 32);
+    orc_options opt;
+    orc_default_options(&opt);
+    ray_t** vrays = (ray_t**)malloc((size_t)ncam * sizeof(ray_t*));
+    double nshade = 0;
+    for (int c = 0; c < ncam; ++c) {
+        vrays[c] = (ray_t*)malloc((size_t)W * H * sizeof(ray_t));
+        const size_t s0 = g_trace_n;
+        for (int y = 0; y < H; ++y)
+            for (int x = 0; x < W; ++x) trace_one(tree, &cams[c], &opt, x, y, &vrays[c][(size_t)y * W + x]);
+        for (size_t i = s0; i < g_trace_n; ++i) nshade += g_trace[i] >> 7;
+    }
+    printf("MEM: %d views %dx%d, %d warps in flight, L2 %.0f MB (%d sectors); %.2fM samples, %.3fM shaded per view\n",
+           ncam, W, H, nw, l2mb, cap, g_trace_n / 1e6 / ncam, nshade / 1e6 / ncam);
+    const int ntx = (W + 3) / 4, nty = (H + 7) / 8;
+    const int groups[5] = {0, ncam, 4, 8, 16};
+    const char* names[5] = {"view-major (parent)", "rows outermost, all views", "rows outermost, groups of 4",
+                            "rows outermost, groups of 8", "rows outermost, groups of 16"};
+    replay_t J[5];
+    pthread_t th[5];
+    for (int k = 0; k < 5; ++k) {
+        memset(&J[k], 0, sizeof(J[k]));
+        J[k].name = names[k]; J[k].vrays = (const ray_t* const*)vrays; J[k].tiles = make_order(ncam, ntx, nty, groups[k]);
+        J[k].ntiles = ncam * ntx * nty; J[k].W = W; J[k].H = H; J[k].nw = nw; J[k].cap = cap;
+        pthread_create(&th[k], NULL, replay, &J[k]);
+    }
+    printf("%-30s %14s %14s %14s %12s %12s\n", "order", "tables MB/fr", "records MB/fr", "DRAM MB/fr", "tbl L2 hit", "rec L2 hit");
+    for (int k = 0; k < 5; ++k) {
+        pthread_join(th[k], NULL);
+        const double tb = J[k].tbl_miss * 32 / 1e6 / ncam, rb = J[k].rec_miss * 32 / 1e6 / ncam;
+        printf("%-30s %14.1f %14.1f %14.1f %11.1f%% %11.1f%%\n", J[k].name, tb, rb, tb + rb,
+               100 * (1 - J[k].tbl_miss / (J[k].tbl_acc + 1e-9)), 100 * (1 - J[k].rec_miss / (3 * J[k].rec_acc + 1e-9)));
+    }
+}
+
 static void report(const char* name, const stats_t* S, int frames) {
     printf("%-34s %7.2f Minstr/frame  body %5.1f/32 (%6.2fM it)  fetch+ %5.1f/32 (%5.2fM)  shade %5.1f/32 (%5.3fM it)\n", name,
            S->instr / frames / 1e6, S->body_lanes / (S->body_iters + 1e-9), S->body_iters / frames / 1e6,
@@ -361,6 +585,16 @@ int main(int argc, char** argv) {
     for (int i = 0; i < 3; ++i) { tree.offset[i] = meta[i]; tree.scale[i] = meta[3 + i]; }
     orc_options opt;
     orc_default_options(&opt);
+    if (getenv("MEM") && atoi(getenv("MEM"))) {   /* L2 replay of the work orders instead of the lane policies */
+        g_mem = 1;
+        orc_camera* oc = (orc_camera*)calloc(ncam, sizeof(orc_camera));
+        for (int c = 0; c < ncam; ++c) {
+            oc[c].width = W; oc[c].height = H; oc[c].fx = meta[6]; oc[c].fy = meta[7];
+            memcpy(oc[c].c2w, cams + 12 * c, 48);
+        }
+        mem_main(&tree, oc, ncam, W, H);
+        return 0;
+    }
 
     stats_t P0 = {0}, P1 = {0}, P2a[6], P2b[6], P3[6];
     memset(P3, 0, sizeof(P3));

@@ -1,6 +1,8 @@
 #!/usr/bin/env python
 """Design tool: dump the bench tree's topology + sigma and a few poses, build tools/lane_sim.c and run
-it.  Ranks lane-scheduling policies of the march kernel on the CPU (no GPU needed)."""
+it.  Ranks lane-scheduling policies of the march kernel on the CPU (no GPU needed).
+MEM=1 replays the DRAM traffic of the batch work orders instead (give it consecutive orbit poses:
+MEM=1 VIEWS=40-71)."""
 import os
 import subprocess
 import sys
@@ -15,7 +17,10 @@ from volrend_b200 import synth  # noqa: E402
 def main():
     depth = int(os.environ.get("DEPTH", 10))
     size = int(os.environ.get("SIZE", 800))
-    views = [int(v) for v in os.environ.get("VIEWS", "0,37,90").split(",")]
+    views = []
+    for v in os.environ.get("VIEWS", "0,37,90").split(","):
+        a, _, b = v.partition("-")
+        views += list(range(int(a), int(b or a) + 1))
     kind = os.environ.get("KIND", "lego")
     dump = f"/tmp/lane_sim_{kind}_{depth}_{size}.bin"
     st = synth.make_tree(kind, depth=depth, basis_dim=1, seed=0)

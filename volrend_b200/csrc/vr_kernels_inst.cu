@@ -54,23 +54,22 @@ void set_work(LaunchDev& P, const LaunchCfg& cfg, bool blocks = true) {
     P.tiles_y = (P.h + kTH - 1) / kTH;
     P.work_counter = cfg.queue;
     // Batches can have the queue hand out blocks of 8x8 tiles, the warps of an SM sharing a block (vr_march.cuh next_item).
-    // Measured: a gain on config 4 (SH25, 160-byte records, 1080p), none on config 2 (SH16): on by default for 25 basis
-    // functions only; VR_BLOCKS=0/1 forces it.  It needs enough blocks
+    // Measured: a gain on config 4 (SH25, 160-byte records, 1080p; still +5 % over single tiles in the rows-across-views
+    // order), none on config 2 (SH16): on for 25 basis functions only.  It needs enough blocks
     // per SM to balance (a block is ~20 us of an SM), so single frames always keep one tile per item.
-    static const int force = getenv("VR_BLOCKS") ? atoi(getenv("VR_BLOCKS")) : -1;
     const long long bx = (P.tiles_x + kBlkW - 1) / kBlkW, by = (P.tiles_y + kBlkH - 1) / kBlkH, nb = bx * by * P.n_views;
-    const bool want = force >= 0 ? force != 0 : (P.tree.kbd == 25 && P.n_views >= 2 && nb >= 16LL * cfg.num_sms);
+    const bool want = P.tree.kbd == 25 && P.n_views >= 2 && nb >= 16LL * cfg.num_sms;
     if (blocks && want && nb * kBlkTiles <= 0x7fffffffLL) {
         P.blk_mode = 1; P.blocks_x = (int)bx; P.n_blocks = (int)nb;
         P.n_tiles = (int)(nb * kBlkTiles);   // item ids (block * 64 + tile), incl. the tiles beyond the image edge
-        set_div((uint32_t)(bx * by), P.div_view_mul, P.div_view_shift);
-        set_div((uint32_t)bx, P.div_row_mul, P.div_row_shift);
+        set_div((uint32_t)bx, P.div_row_mul, P.div_row_shift);   // block -> (block row, view) pair
+        set_div((uint32_t)P.n_views, P.div_view_mul, P.div_view_shift);
         return;
     }
     P.blk_mode = 0; P.blocks_x = 0; P.n_blocks = 0;
     P.n_tiles = P.tiles_x * P.tiles_y * P.n_views;
-    set_div((uint32_t)(P.tiles_x * P.tiles_y), P.div_view_mul, P.div_view_shift);
-    set_div((uint32_t)P.tiles_x, P.div_row_mul, P.div_row_shift);
+    set_div((uint32_t)P.tiles_x, P.div_row_mul, P.div_row_shift);    // item -> (tile row, view) pair (decode_item)
+    set_div((uint32_t)P.n_views, P.div_view_mul, P.div_view_shift);
 }
 
 template <typename K>

@@ -7,7 +7,7 @@
 //   descent   descend_wide (vr_probe.h), restarted at the deepest table the thread's previous point also went
 //             through: the tables of a descent are kept in shared memory, and the first position bit in which the
 //             two points differ bounds how far down the old path is still valid.
-//   records   read like the march reads them (load_rec: L1 no_allocate, L2 evict_first).
+//   records   read like the march reads them (load_rec: plain read-only loads).
 //   rows      a data row is 3*B+1 halves (98 bytes for SH16, 26 for SH4): the warp stages its 32 rows in shared
 //             memory and writes them as one contiguous span of 16-byte stores.
 #include <cuda_fp16.h>

@@ -117,7 +117,7 @@ struct LaunchDev {
     cudaSurfaceObject_t surf, dsurf;
     int32_t composite;     // 1: read existing colour from rgba8/surf + depth limit
     int32_t tiles_x, tiles_y, n_tiles;  // persistent kernels: work decomposition
-    // division of a tile index (< 2^31) by tiles_x*tiles_y and by tiles_x as multiply-high + shift
+    // division of a work item (< 2^31) by tiles_x and of the quotient by n_views as multiply-high + shift
     // (set_div): q = shift < 0 ? n : umulhi(n, mul) >> shift
     uint32_t div_view_mul, div_row_mul;
     int32_t div_view_shift, div_row_shift;
