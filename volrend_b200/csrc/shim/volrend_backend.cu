@@ -11,7 +11,11 @@
 //   volrend::cuda_assert             include/volrend/cuda/common.cuh:78-79 (abort-on-error
 //                                    semantics of src/cuda/common.cu:8-21 are preserved here;
 //                                    the C-ABI underneath never aborts)
-//   volrend::VolumeRenderer          include/volrend/renderer.hpp:11-42, GL-free offscreen Impl
+//   volrend::VolumeRenderer          include/volrend/renderer.hpp:11-42, GL-free Impl: the offscreen march, or
+//                                    with meshes, the probe cube or the grid the mesh pass of
+//                                    cuda_renderer.cpp:83-126 (volrend::Mesh: mesh_b200.cpp)
+#include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -26,6 +30,7 @@
 
 #include "volrend_b200.h"
 #include "volrend_b200_shim.hpp"
+#include "mesh_pass_b200.hpp"
 
 namespace volrend {
 
@@ -182,14 +187,36 @@ struct OffscreenTarget {   // what volrend_b200_read_pixels needs to see of an I
     cudaStream_t stream = nullptr;
     int w = 0, h = 0;
 };
+
+// GL's clear of the mesh framebuffer: colour (bg, bg, bg, 255) and ray distance 1e9
+__global__ void clear_mesh_target(uint32_t* rgba, float* depth, size_t n, uint32_t rgba_word) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        rgba[i] = rgba_word;
+        depth[i] = 1e9f;
+    }
+}
 }  // namespace
 
 struct VolumeRenderer::Impl : OffscreenTarget {
-    Impl(Camera& camera, RenderOptions& options) : camera(camera), options(options) {
+    Impl(Camera& camera, RenderOptions& options, std::vector<Mesh>& meshes)
+        : camera(camera), options(options), meshes(meshes) {
         cuda(StreamCreateWithFlags(&stream, cudaStreamDefault));
+        // the probe marker of cuda_renderer.cpp:25-38: black, faces -z/+z blue, -y/+y green, -x/+x red
+        probe_ = Mesh::Cube(glm::vec3(0.f));
+        probe_.name = "_probe_cube";
+        probe_.visible = false;
+        probe_.scale = 0.05f;
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 12; ++j) probe_.vert[(size_t)(12 * i + j) * 9 + 3 + 2 - i] = 1.f;
+        probe_.unlit = true;
+        probe_.update();
     }
     ~Impl() {
         if (array) cudaFreeArray(array);
+        if (depth_array_) cudaFreeArray(depth_array_);
+        if (rgba_lin_) cudaFree(rgba_lin_);
+        if (depth_lin_) cudaFree(depth_lin_);
+        if (wire_dev_) cudaFree(wire_dev_);
         cudaStreamDestroy(stream);
     }
     void resize(int width, int height) {
@@ -199,16 +226,138 @@ struct VolumeRenderer::Impl : OffscreenTarget {
         cuda(MallocArray(&array, &cd, width, height, cudaArraySurfaceLoadStore));
         w = width; h = height;
     }
+    void set(N3Tree& t) {
+        tree = &t;
+        probe_.scale = 0.02f / t.scale[0];   // cuda_renderer.cpp:178
+        wire_valid_ = false;
+    }
+    void clear() {
+        tree = nullptr;
+        wire_valid_ = false;
+    }
     void render() {
         camera._update();
         if (!array) resize(camera.width, camera.height);
-        if (tree == nullptr || !tree->is_cuda_loaded()) return;
+        probe_.visible = options.enable_probe;   // cuda_renderer.cpp:94-95
+        for (int i = 0; i < 3; ++i) probe_.translation[i] = options.probe[i];
+        const bool has_tree = tree != nullptr && tree->is_cuda_loaded();
+        bool mesh_pass = probe_.visible || (options.show_grid && has_tree);
+        for (const Mesh& m : meshes) mesh_pass = mesh_pass || m.visible;
+        if (mesh_pass) {
+            render_meshes(has_tree);
+            return;
+        }
+        if (!has_tree) return;
         cudaArray_t depth = nullptr;
         launch_renderer(*tree, camera, options, array, depth, stream, true);
     }
+
+    // cuda_renderer.cpp:83-126: clear, draw the meshes, the probe cube and the grid, composite the volume over them
+    void render_meshes(bool has_tree) {
+        if (camera.width != w || camera.height != h) resize(camera.width, camera.height);
+        ensure_mesh_target();
+        const double bg = std::min(std::max((double)options.background_brightness, 0.0), 1.0);
+        const uint32_t b = (uint32_t)std::nearbyint(bg * 255.0);   // round half to even, as Python's round()
+        const size_t n = (size_t)w * h;
+        if (n) {
+            const int blocks = (int)std::min<size_t>((n + 255) / 256, 4096);
+            clear_mesh_target<<<blocks, 256, 0, stream>>>((uint32_t*)rgba_lin_, depth_lin_, n,
+                                                          b | (b << 8) | (b << 16) | (0xffu << 24));
+            cuda(GetLastError());
+        }
+        b200::MeshPass pass;
+        b200::set_current_mesh_pass(&pass);
+        for (const Mesh& mesh : meshes) mesh.draw(camera.w2c, camera.K);
+        probe_.draw(camera.w2c, camera.K);
+        b200::set_current_mesh_pass(nullptr);
+        if (options.show_grid && has_tree) append_grid(pass);
+        vr_camera c;
+        to_c(camera, c);
+        if (!pass.meshes.empty()) {
+            const int rc = vr_draw_meshes(&c, pass.meshes.data(), (int)pass.meshes.size(), rgba_lin_, depth_lin_,
+                                          (void*)stream);
+            if (rc != VR_OK) die("vr_draw_meshes", rc);
+        }
+        cuda(Memcpy2DToArrayAsync(array, 0, 0, rgba_lin_, 4 * (size_t)w, 4 * (size_t)w, h,
+                                  cudaMemcpyDeviceToDevice, stream));
+        if (has_tree) {
+            cuda(Memcpy2DToArrayAsync(depth_array_, 0, 0, depth_lin_, 4 * (size_t)w, 4 * (size_t)w, h,
+                                      cudaMemcpyDeviceToDevice, stream));
+            launch_renderer(*tree, camera, options, array, depth_array_, stream, false);
+        }
+    }
+
+    // RGBA8 and ray-distance buffers for vr_draw_meshes, and the R32F array launch_renderer composites against
+    void ensure_mesh_target() {
+        if (depth_array_ && target_w_ == w && target_h_ == h) return;
+        if (depth_array_) cuda(FreeArray(depth_array_));
+        if (rgba_lin_) cuda(Free(rgba_lin_));
+        if (depth_lin_) cuda(Free(depth_lin_));
+        cudaChannelFormatDesc cd = cudaCreateChannelDesc(32, 0, 0, 0, cudaChannelFormatKindFloat);
+        cuda(MallocArray(&depth_array_, &cd, w, h, cudaArraySurfaceLoadStore));
+        cuda(Malloc((void**)&rgba_lin_, std::max<size_t>((size_t)4 * w * h, 4)));
+        cuda(Malloc((void**)&depth_lin_, std::max<size_t>((size_t)4 * w * h, 4)));
+        target_w_ = w;
+        target_h_ = h;
+    }
+
+    // The octree grid at grid_max_depth (cuda_renderer.cpp:99-111,182-188), generated on the device into a buffer
+    // kept until the depth changes or the tree is set or cleared; drawn unlit as lines with the identity model.
+    void append_grid(b200::MeshPass& pass) {
+        vr_tree* t = device_tree(*tree);
+        if (!t) return;
+        const int depth = options.grid_max_depth;
+        if (!wire_valid_ || wire_depth_ != depth) {
+            wire_valid_ = false;
+            int64_t n = 0;
+            int rc = vr_tree_wireframe(t, depth, nullptr, 0, &n, (void*)stream);
+            if (rc != VR_OK) die("vr_tree_wireframe", rc);
+            if (n > INT32_MAX) {
+                fprintf(stderr, "volrend_b200: grid at depth %d has %lld vertices; a mesh holds at most %d: "
+                        "not drawn\n", depth, (long long)n, INT32_MAX);
+                return;
+            }
+            if ((size_t)n * 9 > wire_cap_) {
+                if (wire_dev_) cuda(Free(wire_dev_));
+                wire_dev_ = nullptr;
+                cuda(Malloc((void**)&wire_dev_, (size_t)n * 9 * sizeof(float)));
+                wire_cap_ = (size_t)n * 9;
+            }
+            int64_t got = 0;
+            if (n) {
+                rc = vr_tree_wireframe(t, depth, wire_dev_, n, &got, (void*)stream);
+                if (rc != VR_OK) die("vr_tree_wireframe", rc);
+            }
+            wire_n_ = n;
+            wire_depth_ = depth;
+            wire_valid_ = true;
+        }
+        if (wire_n_ == 0) return;
+        vr_mesh_desc d;
+        memset(&d, 0, sizeof(d));
+        d.vert_dev = wire_dev_;
+        d.n_verts = (int32_t)wire_n_;
+        d.face_size = 2;
+        d.unlit = 1;
+        for (int i = 0; i < 4; ++i) d.model[5 * i] = 1.f;
+        pass.meshes.push_back(d);
+    }
+
     Camera& camera;
     RenderOptions& options;
+    std::vector<Mesh>& meshes;
     N3Tree* tree = nullptr;
+
+    Mesh probe_;
+    cudaArray_t depth_array_ = nullptr;   // R32F ray distance for launch_renderer(offscreen=false)
+    uint8_t* rgba_lin_ = nullptr;
+    float* depth_lin_ = nullptr;
+    int target_w_ = 0, target_h_ = 0;
+    float* wire_dev_ = nullptr;           // the grid's vertices, wire_n_ of them, for grid_max_depth wire_depth_
+    size_t wire_cap_ = 0;
+    int64_t wire_n_ = 0;
+    int wire_depth_ = 0;
+    bool wire_valid_ = false;             // false: no grid generated
 };
 
 namespace {
@@ -218,7 +367,7 @@ std::unordered_map<const VolumeRenderer*, OffscreenTarget*>& impls() {
 }
 }  // namespace
 
-VolumeRenderer::VolumeRenderer() : impl_(std::make_unique<Impl>(camera, options)) {
+VolumeRenderer::VolumeRenderer() : impl_(std::make_unique<Impl>(camera, options, meshes)) {
     std::lock_guard<std::mutex> lk(g_mu);
     impls()[this] = impl_.get();
 }
@@ -228,12 +377,12 @@ VolumeRenderer::~VolumeRenderer() {
 }
 void VolumeRenderer::render() { impl_->render(); }
 void VolumeRenderer::set(N3Tree& tree) {
-    impl_->tree = &tree;
+    impl_->set(tree);
     // cuda_renderer.cpp:176-177
     options.basis_minmax[0] = 0;
     options.basis_minmax[1] = std::max(tree.data_format.basis_dim - 1, 0);
 }
-void VolumeRenderer::clear() { impl_->tree = nullptr; }
+void VolumeRenderer::clear() { impl_->clear(); }
 void VolumeRenderer::resize(int width, int height) {
     camera.width = width;
     camera.height = height;
