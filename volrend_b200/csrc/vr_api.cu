@@ -18,6 +18,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -44,8 +45,9 @@ std::atomic<int> g_max_ctas{0};
 constexpr int kVariantQueue = 7, kVariantInline = 3 + 16 * 193;
 constexpr int kQueueSlots = 256;
 constexpr int kCamRing = 8192;  // device ring of per-view cameras for batched launches
+}  // namespace
 
-int fail(int code, const char* fmt, ...) {
+int vrb::fail(int code, const char* fmt, ...) {
     char buf[512];
     va_list ap;
     va_start(ap, fmt);
@@ -54,22 +56,64 @@ int fail(int code, const char* fmt, ...) {
     g_err = buf;
     return code;
 }
-#define VR_CUDA(expr)                                                                              \
-    do {                                                                                           \
-        cudaError_t e__ = (expr);                                                                  \
-        if (e__ != cudaSuccess)                                                                    \
-            return fail(e__ == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "%s: %s (%s:%d)", \
-                        #expr, cudaGetErrorString(e__), __FILE__, __LINE__);                       \
+
+namespace {
+// A failed CUDA call: VR_ENOMEM for an allocation, else VR_ECUDA, with the message "<what>: <CUDA's text><where>".
+// The runtime's last error is cleared, so that a later launch check does not report this failure again.
+int cuda_fail(cudaError_t e, const char* what, const char* where = "") {
+    cudaGetLastError();
+    return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "%s: %s%s", what, cudaGetErrorString(e), where);
+}
+#define VR_STR_(x) #x
+#define VR_STR(x) VR_STR_(x)
+#define VR_CUDA(expr)                                                                                    \
+    do {                                                                                                 \
+        const cudaError_t e__ = (expr);                                                                  \
+        if (e__ != cudaSuccess) return cuda_fail(e__, #expr, " (" __FILE__ ":" VR_STR(__LINE__) ")"); \
     } while (0)
+
+// f(std::integral_constant<int, K>{}) for the kernel bases K the march kernels are built for (vr_kernels_inst.cu, one
+// object per entry of the Makefile's KBDS); `otherwise` for any other kbd.
+template <class R, class F>
+R with_kbd(int kbd, R otherwise, F f) {
+    switch (kbd) {
+        case -1: return f(std::integral_constant<int, -1>{});
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 4: return f(std::integral_constant<int, 4>{});
+        case 9: return f(std::integral_constant<int, 9>{});
+        case 16: return f(std::integral_constant<int, 16>{});
+        case 25: return f(std::integral_constant<int, 25>{});
+        default: return otherwise;
+    }
+}
 
 int kernel_basis(int format, int basis_dim) {
     if (format == VR_FMT_RGBA || basis_dim < 0) return -1;
-    switch (basis_dim) {
-        case 1: case 4: case 9: case 16: case 25: return basis_dim;
-        default: return 1;  // rt_core.cuh:134-160: no switch case matches -> only coefficient 0
-    }
+    // rt_core.cuh:134-160: no switch case matches -> only coefficient 0
+    return with_kbd(basis_dim, 1, [](auto k) { return decltype(k)::value; });
 }
 int rec_bytes_for(int kbd) { return kbd <= 1 ? 8 : ((3 * kbd * 2 + 15) / 16) * 16; }
+
+// All views of a batch have view 0's image size.
+int same_size(const vr_camera* cams, int n_views) {
+    for (int v = 1; v < n_views; ++v)
+        if (cams[v].width != cams[0].width || cams[v].height != cams[0].height)
+            return fail(VR_EINVAL, "view %d is %dx%d, view 0 %dx%d: all views of a batch must share one image size", v,
+                        cams[v].width, cams[v].height, cams[0].width, cams[0].height);
+    return VR_OK;
+}
+
+// Calls f(v0, nv) for consecutive chunks [v0, v0 + nv) of at most max_views views; stops at the first error.
+template <class F>
+int for_chunks(int n_views, int max_views, F f) {
+    for (int v0 = 0; v0 < n_views; v0 += max_views)
+        if (int rc = f(v0, std::min(max_views, n_views - v0))) return rc;
+    return VR_OK;
+}
+
+// p advanced by n elements; a null (absent) output stays null.
+template <class T>
+T* skip(T* p, size_t n) { return p ? p + n : p; }
 }  // namespace
 
 // Per-stream launch resources of a tree.  Work-queue slots and the camera ring are recycled in
@@ -118,6 +162,33 @@ struct vr_tree {
     bool wire_ready = false;
     WireLevels wire_levels{};
 };
+
+namespace {
+// The device check of every entry point.  With a tree, the current device must be the tree's (cudaGetDevice only, so
+// launches pay no more); without one, some device must exist.
+int need_device(const vr_tree* t) {
+    int dev = -1, ndev = 0;
+    const bool ok = t ? cudaGetDevice(&dev) == cudaSuccess
+                      : cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && cudaGetDevice(&dev) == cudaSuccess;
+    if (!ok) {
+        cudaGetLastError();
+        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
+    }
+    if (t && dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
+    return VR_OK;
+}
+
+// The tree's basis has no kernel of its own (kernel_basis): the device keeps only coefficient 0 of each channel.
+bool coef0_only(const vr_tree* t) { return t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim; }
+
+// opt's basis_minmax clamped to the tree's basis, as the march clamps it (NULL opt: the whole basis).  The reference
+// sums basis_minmax[0]..[1] and reads past the coefficients when the range leaves the tree's basis.
+void basis_range(const vr_tree* t, const vr_options* opt, int32_t* bmin, int32_t* bmax) {
+    const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
+    *bmin = opt ? std::max(opt->basis_minmax[0], 0) : 0;
+    *bmax = opt ? std::min(opt->basis_minmax[1], nb - 1) : nb - 1;
+}
+}  // namespace
 
 // ------------------------------------------------------------------------------------ upload
 namespace {
@@ -401,21 +472,13 @@ extern "C" {
 const char* vr_last_error(void) { return g_err.c_str(); }
 const char* vr_version(void) { return "volrend_b200 0.2 (sm_90a)"; }
 static bool variant_ok(int kbd, int variant) {
-    switch (kbd) {
-        case -1: return variant_supported<-1>(variant);
-        case 1: return variant_supported<1>(variant);
-        case 4: return variant_supported<4>(variant);
-        case 9: return variant_supported<9>(variant);
-        case 16: return variant_supported<16>(variant);
-        case 25: return variant_supported<25>(variant);
-        default: return false;
-    }
+    return with_kbd(kbd, false, [&](auto k) { return variant_supported<decltype(k)::value>(variant); });
 }
 int vr_variant_supported(int kernel_basis, int variant) { return variant >= 0 && variant_ok(kernel_basis, variant) ? 1 : 0; }
 int vr_set_variant(int variant) {
     // accepted when at least one basis size has it; a tree whose basis size lacks it fails at launch
     bool any = false;
-    for (int kbd : {-1, 1, 4, 9, 16, 25}) any = any || (variant >= 0 && variant_ok(kbd, variant));
+    for (int kbd = -1; kbd <= VR_BASIS_MAX; ++kbd) any = any || (variant >= 0 && variant_ok(kbd, variant));
     if (!any) return fail(VR_EINVAL, "kernel variant %d is not built into this library", variant);
     g_variant.store(variant);
     return VR_OK;
@@ -466,11 +529,7 @@ void vr_tree_destroy(vr_tree* t) {
 static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, vr_tree** out) {
     if (!d || !out) return fail(VR_EINVAL, "null argument");
     *out = nullptr;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
-    }
+    if (int rc = need_device(nullptr)) return rc;
     if (d->N != 2) return fail(VR_EUNSUPPORTED, "N=%d: only N=2 octrees are supported (as in the reference)", d->N);
     if (d->capacity < 1 || d->capacity >= (1ll << 28)) return fail(VR_EINVAL, "capacity %lld out of range", (long long)d->capacity);
     if (!d->child || (!q && !d->data)) return fail(VR_EINVAL, "child/data arrays missing");
@@ -616,11 +675,12 @@ static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, 
     release(depth);
     {
         const size_t wrec_bytes = (size_t)n_entries * rec_bytes;
-        cudaError_t e = cudaMalloc(&t->wrecs, wrec_bytes);
+        const cudaError_t e = cudaMalloc(&t->wrecs, wrec_bytes);
         if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(VR_ENOMEM, "colour records of the wide tables need %.2f GB (%lld entries x %d B): %s", wrec_bytes / 1e9,
-                        n_entries, rec_bytes, cudaGetErrorString(e));
+            char what[128];
+            snprintf(what, sizeof(what), "colour records of the wide tables need %.2f GB (%lld entries x %d B)",
+                     wrec_bytes / 1e9, n_entries, rec_bytes);
+            return cuda_fail(e, what);
         }
         const long long rwork = n_entries * (rec_bytes >= 16 ? rec_bytes / 16 : 1);
         build_wrecs_kernel<<<(unsigned)((rwork + TB - 1) / TB), TB>>>(t->wslot, S, t->wrecs, n_entries, rec_bytes);
@@ -754,14 +814,9 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
     }
     cfg.pool = nullptr; cfg.pool_bytes = 0;
     if ((cfg.variant & 15) == 8) {   // ray-pool kernel: its parked-ray stacks live with the (tree, stream) resources
-        size_t need = 0;
-        switch (t->dev.kbd) {
-            case 4: need = pool_bytes_for<4>(t->num_sms, t->dev.max_depth); break;
-            case 9: need = pool_bytes_for<9>(t->num_sms, t->dev.max_depth); break;
-            case 16: need = pool_bytes_for<16>(t->num_sms, t->dev.max_depth); break;
-            case 25: need = pool_bytes_for<25>(t->num_sms, t->dev.max_depth); break;
-            default: break;
-        }
+        const size_t need = with_kbd(t->dev.kbd, size_t(0), [&](auto k) {
+            return pool_bytes_for<decltype(k)::value>(t->num_sms, t->dev.max_depth);
+        });
         std::lock_guard<std::mutex> lk(mt->res_mu);
         if (need > sr->pool_bytes) {
             // a grow only happens before the first kind-8 launch on this stream (the size depends on the tree alone)
@@ -775,16 +830,10 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
     cfg.l2_window_bytes = t->l2_window_bytes;
     static const bool no_pdl = getenv("VR_NO_PDL") != nullptr && atoi(getenv("VR_NO_PDL")) > 0;
     cfg.pdl = !no_pdl;
-    cudaError_t e;
-    switch (t->dev.kbd) {
-        case -1: e = launch_march<-1>(P, cfg); break;
-        case 1: e = launch_march<1>(P, cfg); break;
-        case 4: e = launch_march<4>(P, cfg); break;
-        case 9: e = launch_march<9>(P, cfg); break;
-        case 16: e = launch_march<16>(P, cfg); break;
-        case 25: e = launch_march<25>(P, cfg); break;
-        default: return fail(VR_EUNSUPPORTED, "unsupported kernel basis %d", t->dev.kbd);
-    }
+    // variant_ok above has rejected every kbd without kernels
+    const cudaError_t e = with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
+        return launch_march<decltype(k)::value>(P, cfg);
+    });
     if (e != cudaSuccess) return fail(VR_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     g_launches += 1;
     return VR_OK;
@@ -806,15 +855,9 @@ int check_common(const vr_tree* t, const vr_camera* cam, const vr_options* opt, 
     }
     if (tile_bound(r) > 0x7fffffffLL)
         return fail(VR_EUNSUPPORTED, "%dx%d pixels: more tiles than the 31-bit work queue can index", r.w, r.h);
-    int dev = -1;
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(VR_ENODEVICE, "no CUDA device");
-    if (dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
-    return VR_OK;
+    return need_device(t);
 }
 
-}  // namespace
-
-namespace {
 // Cameras of a batch go through a device ring owned by (tree, stream): no allocation on the launch path (a
 // stream-ordered pool would hand memory back to the OS at every synchronisation), and a slot is rewritten
 // only by a copy that is stream-ordered behind the launch that read it.  n_views <= kCamRing.
@@ -849,24 +892,53 @@ int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_
     }
     return VR_OK;
 }
+
+// The march launches of every render entry point.  P holds the outputs and the rect (x0, y0, w, h; the output buffers
+// hold h rows of w pixels per view); this adds the tree, the cameras and the options, and launches the views in chunks
+// that fit the camera ring and the 31-bit tile index, the output pointers advanced to each chunk's first view.
+// opt_stride as in vr_frames.h; a chunk of one view is an ordinary single-view launch with that view's options.
+int march(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
+          const LaunchDev& P, bool surface, cudaStream_t stream) {
+    const long long tb = tile_bound(vr_rect{P.x0, P.y0, P.w, P.h});
+    const int max_views = tb * kCamRing > 0x7fffffffLL ? (int)(0x7fffffffLL / tb) : kCamRing;
+    const size_t px = (size_t)P.w * P.h;
+    return for_chunks(n_views, max_views, [&](int v0, int nv) {
+        const vr_options* o = opt + (size_t)opt_stride * v0;
+        LaunchDev C = P;
+        C.tree = t->dev;
+        fill_opt(C.opt, o);
+        fill_cam(C.cam, &cams[v0]);
+        C.n_views = nv;
+        C.rgba8 = skip(P.rgba8, 4 * px * v0);
+        C.rgbaf = skip(P.rgbaf, px * v0);
+        C.depth_in = skip(P.depth_in, px * v0);
+        if (int rc = stage_cams(t, cams + v0, nv, stream, C, opt_stride ? o : nullptr)) return rc;
+        return dispatch(t, C, P.counters != nullptr, surface, stream);
+    });
+}
+
+// vr_render_composite_batch (opt_stride 0) and vr_render_composite_batch_opts (opt_stride 1)
+int render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
+                           const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev, float* rgba32f_dev,
+                           void* stream) {
+    if (n_views > 0 && (!rgba8_dev || !depth_dev)) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
+    return render_batch(t, cams, n_views, opt, opt_stride, tile, rgba8_dev, rgba32f_dev, nullptr, stream, depth_dev);
+}
 }  // namespace
 
 namespace vrb {
 
 // vr_render_batch (opt_stride 0: one options struct for every view) and vr_render_batch_opts (opt_stride 1: view i
-// uses opt[i]).  A batch of one view is an ordinary single-view launch with that view's options.
+// uses opt[i]).
 int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
-                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream_,
+                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream,
                  const float* depth_dev) {
-    cudaStream_t stream = (cudaStream_t)stream_;
     if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
     if (n_views == 0) return VR_OK;
     vr_rect r;
     int rc = check_common(t, cams, opt, tile, r);
     if (rc) return rc;
-    for (int i = 1; i < n_views; ++i)
-        if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
-            return fail(VR_EINVAL, "all views of a batch must share one image size");
+    if ((rc = same_size(cams, n_views))) return rc;
     if (depth_dev && !rgba8_dev) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
     const bool per_view = opt_stride != 0 && n_views > 1;
     if ((per_view || depth_dev) && n_views > 1) {
@@ -878,30 +950,11 @@ int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_
     }
     if (r.w == 0 || r.h == 0) return VR_OK;
     LaunchDev P{};
-    P.tree = t->dev;
-    fill_opt(P.opt, opt);
-    fill_cam(P.cam, &cams[0]);
-    P.n_views = n_views;
     P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
     P.rgba8 = rgba8_dev; P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
     P.counters = counters_dev;
     P.depth_in = depth_dev; P.composite = depth_dev != nullptr;
-    int max_views = kCamRing;  // split very large batches: camera ring size, 31-bit tile index
-    if (tile_bound(r) * max_views > 0x7fffffffLL) max_views = (int)(0x7fffffffLL / tile_bound(r));
-    if (n_views > max_views) {
-        const size_t tile_px = (size_t)r.w * r.h;
-        for (int v0 = 0; v0 < n_views; v0 += max_views) {
-            const int nv = n_views - v0 < max_views ? n_views - v0 : max_views;
-            rc = render_batch(t, cams + v0, nv, opt + (size_t)opt_stride * v0, opt_stride, tile,
-                              rgba8_dev ? rgba8_dev + 4 * tile_px * v0 : nullptr,
-                              rgba32f_dev ? rgba32f_dev + 4 * tile_px * v0 : nullptr, counters_dev, stream_,
-                              depth_dev ? depth_dev + tile_px * v0 : nullptr);
-            if (rc) return rc;
-        }
-        return VR_OK;
-    }
-    if ((rc = stage_cams(t, cams, n_views, stream, P, per_view ? opt : nullptr))) return rc;
-    return dispatch(t, P, counters_dev != nullptr, false, stream);
+    return march(t, cams, n_views, opt, opt_stride, P, false, (cudaStream_t)stream);
 }
 
 }  // namespace vrb
@@ -922,19 +975,17 @@ int vr_render_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, c
 int vr_render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
                               const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev, float* rgba32f_dev,
                               void* stream) {
-    if (n_views > 0 && (!rgba8_dev || !depth_dev)) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
-    return render_batch(t, cams, n_views, opt, 0, tile, rgba8_dev, rgba32f_dev, nullptr, stream, depth_dev);
+    return render_composite_batch(t, cams, n_views, opt, 0, tile, rgba8_dev, depth_dev, rgba32f_dev, stream);
 }
 
 int vr_render_composite_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opts,
                                    const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev,
                                    float* rgba32f_dev, void* stream) {
-    if (n_views > 0 && (!rgba8_dev || !depth_dev)) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
-    return render_batch(t, cams, n_views, opts, 1, tile, rgba8_dev, rgba32f_dev, nullptr, stream, depth_dev);
+    return render_composite_batch(t, cams, n_views, opts, 1, tile, rgba8_dev, depth_dev, rgba32f_dev, stream);
 }
 
 int vr_render_bands_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int band_h,
-                          int n_parts, int part, uint8_t* rgba8_dev, float* rgba32f_dev, void* stream_) {
+                          int n_parts, int part, uint8_t* rgba8_dev, float* rgba32f_dev, void* stream) {
     if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
     if (n_views == 0) return VR_OK;
     vr_rect r;
@@ -942,35 +993,14 @@ int vr_render_bands_batch(const vr_tree* t, const vr_camera* cams, int n_views, 
     if (rc) return rc;
     if (band_h < 4 || band_h % 4 || n_parts < 1 || part < 0 || part >= n_parts)
         return fail(VR_EINVAL, "bands: band_h must be a positive multiple of 4 and 0 <= part < n_parts");
-    for (int i = 1; i < n_views; ++i)
-        if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
-            return fail(VR_EINVAL, "all views of a batch must share one image size");
+    if ((rc = same_size(cams, n_views))) return rc;
     const int rows = vr_band_rows(cams[0].height, band_h, n_parts, part);
     if (rows == 0) return VR_OK;
-    vr_rect rr = r;
-    rr.h = rows;
-    int max_views = kCamRing;  // camera ring size, 31-bit tile index
-    if (tile_bound(rr) * max_views > 0x7fffffffLL) max_views = (int)(0x7fffffffLL / tile_bound(rr));
-    if (n_views > max_views) {
-        const size_t part_px = (size_t)r.w * rows;
-        for (int v0 = 0; v0 < n_views; v0 += max_views) {
-            const int nv = n_views - v0 < max_views ? n_views - v0 : max_views;
-            rc = vr_render_bands_batch(t, cams + v0, nv, opt, band_h, n_parts, part, rgba8_dev ? rgba8_dev + 4 * part_px * v0 : nullptr,
-                                       rgba32f_dev ? rgba32f_dev + 4 * part_px * v0 : nullptr, stream_);
-            if (rc) return rc;
-        }
-        return VR_OK;
-    }
     LaunchDev P{};
-    P.tree = t->dev;
-    fill_opt(P.opt, opt);
-    fill_cam(P.cam, &cams[0]);
-    P.n_views = n_views;
-    P.x0 = 0; P.y0 = 0; P.w = r.w; P.h = rows;
+    P.w = r.w; P.h = rows;
     P.band_h = band_h; P.band_parts = n_parts; P.band_part = part;
     P.rgba8 = rgba8_dev; P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
-    if ((rc = stage_cams(t, cams, n_views, (cudaStream_t)stream_, P))) return rc;
-    return dispatch(t, P, false, false, (cudaStream_t)stream_);
+    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream);
 }
 
 int vr_render_bands(const vr_tree* t, const vr_camera* cam, const vr_options* opt, int band_h, int n_parts,
@@ -990,19 +1020,15 @@ int vr_band_rows(int height, int band_h, int n_parts, int part) {
 }
 
 int vr_debug_trace(const vr_tree* t, const vr_camera* cam, const vr_options* opt, uint8_t* rgba8_dev,
-                   vr_counters* counters_dev, unsigned long long* trace_dev, void* stream_) {
+                   vr_counters* counters_dev, unsigned long long* trace_dev, void* stream) {
     vr_rect r;
     int rc = check_common(t, cam, opt, nullptr, r);
     if (rc) return rc;
     if (!counters_dev || !trace_dev) return fail(VR_EINVAL, "trace needs counters and a trace buffer");
     LaunchDev P{};
-    P.tree = t->dev;
-    fill_opt(P.opt, opt);
-    fill_cam(P.cam, cam);
-    P.n_views = 1;
-    P.x0 = 0; P.y0 = 0; P.w = r.w; P.h = r.h;
+    P.w = r.w; P.h = r.h;
     P.rgba8 = rgba8_dev; P.counters = counters_dev; P.trace = trace_dev;
-    return dispatch(t, P, true, false, (cudaStream_t)stream_);
+    return march(t, cam, 1, opt, 0, P, false, (cudaStream_t)stream);
 }
 
 int vr_render(const vr_tree* t, const vr_camera* cam, const vr_options* opt, const vr_rect* tile, uint8_t* rgba8_dev,
@@ -1016,20 +1042,16 @@ int vr_render_composite(const vr_tree* t, const vr_camera* cam, const vr_options
 }
 
 int vr_render_surface(const vr_tree* t, const vr_camera* cam, const vr_options* opt, unsigned long long rgba8_surf,
-                      unsigned long long depth_surf, void* stream_) {
+                      unsigned long long depth_surf, void* stream) {
     vr_rect r;
     int rc = check_common(t, cam, opt, nullptr, r);
     if (rc) return rc;
     if (!rgba8_surf) return fail(VR_EINVAL, "null surface");
     LaunchDev P{};
-    P.tree = t->dev;
-    fill_opt(P.opt, opt);
-    fill_cam(P.cam, cam);
-    P.n_views = 1;
-    P.x0 = 0; P.y0 = 0; P.w = r.w; P.h = r.h;
+    P.w = r.w; P.h = r.h;
     P.surf = (cudaSurfaceObject_t)rgba8_surf; P.dsurf = (cudaSurfaceObject_t)depth_surf;
     P.composite = depth_surf != 0;
-    return dispatch(t, P, false, true, (cudaStream_t)stream_);
+    return march(t, cam, 1, opt, 0, P, true, (cudaStream_t)stream);
 }
 
 }  // extern "C"
@@ -1046,9 +1068,7 @@ int vrb::render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views
     vr_rect r;
     int rc = check_common(t, cams, opt, nullptr, r);
     if (rc) return rc;
-    for (int i = 1; i < n_views; ++i)
-        if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
-            return fail(VR_EINVAL, "all views must share one image size");
+    if ((rc = same_size(cams, n_views))) return rc;
     const size_t frame = (size_t)4 * r.w * r.h;
     int chunk = 8;
     if (const char* e = getenv("VR_HOST_CHUNK")) chunk = atoi(e) > 0 ? atoi(e) : chunk;
@@ -1145,10 +1165,8 @@ int vr_copy2d_async(void* dst, size_t dpitch, const void* src, size_t spitch, si
 
 int vr_probe_lumisphere(const vr_tree* t, const float xyz[3], float* out_dev, void* stream_) {
     if (!t || !xyz || !out_dev) return fail(VR_EINVAL, "null argument");
-    int dev = -1;
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(VR_ENODEVICE, "no CUDA device");
-    if (dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
-    if (t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim)
+    if (int rc = need_device(t)) return rc;
+    if (coef0_only(t))
         return fail(VR_EUNSUPPORTED, "probe unavailable for basis_dim %d (only coefficient 0 is resident)", t->dev.basis_dim);
     // the resident record holds the colour coefficients only: 3 per RGBA leaf, 3*basis_dim otherwise
     // (extra trailing channels of an over-wide data_dim are not kept)
@@ -1170,11 +1188,9 @@ static int query_check(const vr_tree* t, const float* xyz, int64_t n, bool* full
     if (!t) return fail(VR_EINVAL, "null tree");
     if (n < 0) return fail(VR_EINVAL, "n = %lld < 0", (long long)n);
     if (!xyz && n > 0) return fail(VR_EINVAL, "null points with n = %lld", (long long)n);
-    int dev = -1;
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(VR_ENODEVICE, "no CUDA device");
-    if (dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
+    if (int rc = need_device(t)) return rc;
     const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
-    *full = !(t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim) && t->data_dim == 3 * nb + 1;
+    *full = !coef0_only(t) && t->data_dim == 3 * nb + 1;
     return VR_OK;
 }
 
@@ -1201,8 +1217,8 @@ int vr_tree_query(const vr_tree* t, const float* xyz_dev, int64_t n, uint16_t* d
     if (rc) return rc;
     if (data_dev && !full)
         return fail(VR_EUNSUPPORTED, "data rows unavailable for basis_dim %d, data_dim %d (the device keeps %s)",
-                    t->dev.basis_dim, t->data_dim, t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim
-                    ? "only coefficient 0" : "the colour coefficients and sigma only");
+                    t->dev.basis_dim, t->data_dim,
+                    coef0_only(t) ? "only coefficient 0" : "the colour coefficients and sigma only");
     if (n == 0 || (!data_dev && !cube_dev && !local_dev)) return VR_OK;
     int bc;
     if ((bc = query_buffer_check(t, xyz_dev, "xyz_dev")) || (bc = query_buffer_check(t, data_dev, "data_dev")) ||
@@ -1224,7 +1240,7 @@ int vr_tree_eval(const vr_tree* t, const float* xyz_dev, const float* dir_dev, i
     const int rc = query_check(t, xyz_dev, n, &full);
     if (rc) return rc;
     if (rgb_dev && !dir_dev && n > 0) return fail(VR_EINVAL, "null directions with n = %lld", (long long)n);
-    if (rgb_dev && t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim)
+    if (rgb_dev && coef0_only(t))
         return fail(VR_EUNSUPPORTED, "eval unavailable for basis_dim %d (only coefficient 0 is resident)", t->dev.basis_dim);
     if (n == 0 || (!rgb_dev && !sigma_dev)) return VR_OK;
     int bc;
@@ -1235,10 +1251,7 @@ int vr_tree_eval(const vr_tree* t, const float* xyz_dev, const float* dir_dev, i
     Q.tree = t->dev;
     Q.xyz = xyz_dev; Q.dir = dir_dev; Q.n = n;
     Q.rgb = rgb_dev; Q.sigma = sigma_dev;
-    // as vr_draw_probe: basis_minmax clamped to the tree's basis (NULL opt: the whole basis)
-    const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
-    Q.bmin = opt ? std::max(opt->basis_minmax[0], 0) : 0;
-    Q.bmax = opt ? std::min(opt->basis_minmax[1], nb - 1) : nb - 1;
+    basis_range(t, opt, &Q.bmin, &Q.bmax);
     VR_CUDA(query_launch(Q, t->dev.kbd, true, t->num_sms, (cudaStream_t)stream_));
     g_launches += 1;
     return VR_OK;
@@ -1260,10 +1273,8 @@ int vr_draw_probe(const vr_tree* t, const vr_camera* cams, int n_views, const vr
     vr_rect r;
     int rc = check_common(t, cams, opt, tile, r);
     if (rc) return rc;
-    for (int i = 1; i < n_views; ++i)
-        if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
-            return fail(VR_EINVAL, "all views of a batch must share one image size");
-    if (t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim)
+    if ((rc = same_size(cams, n_views))) return rc;
+    if (coef0_only(t))
         return fail(VR_EUNSUPPORTED, "probe unavailable for basis_dim %d (only coefficient 0 is resident)", t->dev.basis_dim);
     if (disp_size <= 0) return VR_OK;   // the reference's candidate pixels then all lie outside the disc
     // candidate corner, volrend.cu:100-101: y < S + 5 && x >= W - S - 5, in the 32-bit wrapping adds of the SASS
@@ -1272,39 +1283,30 @@ int vr_draw_probe(const vr_tree* t, const vr_camera* cams, int n_views, const vr
     const int cx0 = std::max(std::max(x_beg, 0), r.x0), cx1 = std::min(W, r.x0 + r.w);
     const int cy0 = r.y0, cy1 = std::min(std::min(y_end, H), r.y0 + r.h);
     if (cx0 >= cx1 || cy0 >= cy1) return VR_OK;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    if (n_views > kCamRing) {
-        const size_t tile_px = (size_t)r.w * r.h;
-        for (int v0 = 0; v0 < n_views; v0 += kCamRing) {
-            const int nv = n_views - v0 < kCamRing ? n_views - v0 : kCamRing;
-            rc = vr_draw_probe(t, cams + v0, nv, opt, probe_xyz, disp_size, tile, rgba8_dev ? rgba8_dev + 4 * tile_px * v0 : nullptr,
-                               rgba32f_dev ? rgba32f_dev + 4 * tile_px * v0 : nullptr, 0, stream_);
-            if (rc) return rc;
-        }
-        return VR_OK;
-    }
+    const cudaStream_t stream = (cudaStream_t)stream_;
     ProbeLaunch P{};
     P.tree = t->dev;
     for (int i = 0; i < 3; ++i) P.probe[i] = probe_xyz[i];
     P.disp = disp_size;
-    // the reference sums basis_minmax[0]..[1] and reads past the coefficients when the range leaves the tree's
-    // basis; here it is clamped to the basis, as the march clamps it
-    const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
-    P.bmin = std::max(opt->basis_minmax[0], 0);
-    P.bmax = std::min(opt->basis_minmax[1], nb - 1);
-    fill_cam(P.cam, &cams[0]);
-    P.n_views = n_views;
+    basis_range(t, opt, &P.bmin, &P.bmax);
     P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
     P.cx0 = cx0; P.cy0 = cy0; P.cw = cx1 - cx0; P.ch = cy1 - cy0;
-    P.rgba8 = rgba8_dev; P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
     P.surf = (cudaSurfaceObject_t)rgba8_surf;
-    LaunchDev L{};
-    if ((rc = stage_cams(t, cams, n_views, stream, L))) return rc;
-    P.cams = n_views > 1 ? L.cams : nullptr;
-    const cudaError_t e = probe_draw(P, t->dev.kbd, stream);
-    if (e != cudaSuccess) return fail(VR_ECUDA, "probe overlay launch failed: %s", cudaGetErrorString(e));
-    g_launches += 1;
-    return VR_OK;
+    const size_t px = (size_t)r.w * r.h;
+    return for_chunks(n_views, kCamRing, [&](int v0, int nv) -> int {
+        ProbeLaunch C = P;
+        fill_cam(C.cam, &cams[v0]);
+        C.n_views = nv;
+        C.rgba8 = skip(rgba8_dev, 4 * px * v0);
+        C.rgbaf = skip(reinterpret_cast<float4*>(rgba32f_dev), px * v0);
+        LaunchDev L{};
+        if (int rc = stage_cams(t, cams + v0, nv, stream, L)) return rc;
+        C.cams = nv > 1 ? L.cams : nullptr;
+        const cudaError_t e = probe_draw(C, t->dev.kbd, stream);
+        if (e != cudaSuccess) return fail(VR_ECUDA, "probe overlay launch failed: %s", cudaGetErrorString(e));
+        g_launches += 1;
+        return VR_OK;
+    });
 }
 
 // Mesh pass of cuda_renderer.cpp:103-112 without GL (kernels: vr_raster.cu).  The view matrix is
@@ -1334,10 +1336,7 @@ int vr_draw_meshes_batch(const vr_camera* cams, int n_views, const vr_mesh_desc*
     if (W <= 0 || H <= 0) return fail(VR_EINVAL, "zero-size frame %dx%d", W, H);
     if (W > kRasterMaxSide || H > kRasterMaxSide)
         return fail(VR_EINVAL, "frame %dx%d exceeds %d pixels per side", W, H, kRasterMaxSide);
-    for (int v = 1; v < n_views; ++v)
-        if (cams[v].width != W || cams[v].height != H)
-            return fail(VR_EINVAL, "view %d is %dx%d, view 0 %dx%d: all views of a batch must share one image size",
-                        v, cams[v].width, cams[v].height, W, H);
+    if (int rc = same_size(cams, n_views)) return rc;
     const long long npx = (long long)W * H;
     std::vector<RasterMesh> rm;
     std::vector<RasterFrame> rf;
@@ -1406,8 +1405,7 @@ int vr_draw_meshes_batch(const vr_camera* cams, int n_views, const vr_mesh_desc*
         caps.push_back(large_cap);
         first.push_back(m0);
     }
-    int dev = -1;
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
+    if (int rc = need_device(nullptr)) return rc;
     first.push_back(rm.size());
     for (size_t g0 = 0; g0 < rf.size();) {
         // grow the group while it stays within the bounds; a first view that exceeds kRasterScratchBytes alone
@@ -1443,12 +1441,7 @@ int vr_draw_meshes_batch(const vr_camera* cams, int n_views, const vr_mesh_desc*
 int vr_tree_wireframe(const vr_tree* t, int max_depth, float* vert_dev, int64_t max_verts, int64_t* n_verts_out,
                       void* stream_) {
     if (!t || !n_verts_out) return fail(VR_EINVAL, "null argument");
-    int ndev = 0, dev = -1;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cudaGetDevice(&dev) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
-    }
-    if (dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
+    if (int rc = need_device(t)) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     vr_tree* mt = const_cast<vr_tree*>(t);
     WireTree w{};
@@ -1460,8 +1453,7 @@ int vr_tree_wireframe(const vr_tree* t, int max_depth, float* vert_dev, int64_t 
         if (!mt->wire_ready) {
             const cudaError_t e = wire_levels(w, mt->wire_levels, stream, &launches);
             g_launches += launches;
-            if (e != cudaSuccess)
-                return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "wireframe cell count: %s", cudaGetErrorString(e));
+            if (e != cudaSuccess) return cuda_fail(e, "wireframe cell count");
             mt->wire_ready = true;
         }
     }
@@ -1472,8 +1464,7 @@ int vr_tree_wireframe(const vr_tree* t, int max_depth, float* vert_dev, int64_t 
     launches = 0;
     const cudaError_t e = wire_fill(w, t->wire_levels, max_depth, vert_dev, stream, &launches);
     g_launches += launches;
-    if (e != cudaSuccess)
-        return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "wireframe: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return cuda_fail(e, "wireframe");
     return VR_OK;
 }
 
@@ -1487,16 +1478,11 @@ int vr_mesh_estimate_normals(float* vert_dev, int64_t n_verts, const uint32_t* f
     if (n_verts > INT32_MAX) return fail(VR_EINVAL, "%lld vertices: at most %d", (long long)n_verts, INT32_MAX);
     if (faces_dev && n_faces > INT32_MAX / 3)
         return fail(VR_EINVAL, "%lld faces: at most %d face corners", (long long)n_faces, INT32_MAX);
-    int ndev = 0, dev = -1;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cudaGetDevice(&dev) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
-    }
+    if (int rc = need_device(nullptr)) return rc;
     int launches = 0;
     const cudaError_t e = normals_estimate(vert_dev, n_verts, faces_dev, n_faces, (cudaStream_t)stream, &launches);
     g_launches += launches;
-    if (e != cudaSuccess)
-        return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "mesh normals: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return cuda_fail(e, "mesh normals");
     return VR_OK;
 }
 
@@ -1519,11 +1505,7 @@ int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim
         return fail(VR_EINVAL, "null argument");
     if ((n_retain > 0) != (data_retained_dev != nullptr))
         return fail(VR_EINVAL, "data_retained_dev must be NULL exactly when n_retain == 0");
-    int ndev = 0, dev = -1;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cudaGetDevice(&dev) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
-    }
+    if (int rc = need_device(nullptr)) return rc;
     QuantArgs a{};
     a.data = data_dev; a.n_child = n_child; a.data_dim = data_dim; a.n_retain = n_retain; a.bits = bits;
     a.thresh = __half2float(__float2half_rn(sigma_thresh));   // sigma > thresh compared as fp16
@@ -1532,8 +1514,7 @@ int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim
     int reject = kQuantOk, launches = 0;
     const cudaError_t e = quant_compress(a, (cudaStream_t)stream, &kept, &reject, &launches);
     g_launches += launches;
-    if (e != cudaSuccess)
-        return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "tree compress: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return cuda_fail(e, "tree compress");
     if (reject == kQuantNonFinite) return fail(VR_EINVAL, "a quantised coefficient of a kept voxel is Inf or NaN");
     if (reject == kQuantTooManyPoints)
         return fail(VR_EINVAL, "%lld kept voxels x %d quantised basis functions exceed %d points", kept, n_quant, INT32_MAX);

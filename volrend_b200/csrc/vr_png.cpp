@@ -9,8 +9,10 @@
 #include <zlib.h>
 
 #include <atomic>
+#include <cerrno>
 #include <cstdio>
 #include <cstring>
+#include <mutex>
 #include <string>
 #include <thread>
 #include <vector>
@@ -34,8 +36,7 @@ void chunk(std::vector<unsigned char>& out, const char type[4], const unsigned c
     put32(out, crc);
 }
 
-bool encode_png(const uint8_t* rgba, int w, int h, std::vector<unsigned char>& out) {
-    if (!rgba || w <= 0 || h <= 0) return false;
+void encode_png(const uint8_t* rgba, int w, int h, std::vector<unsigned char>& out) {
     const size_t row = (size_t)w * 4, raw_n = (row + 1) * (size_t)h;
     // zlib stream of stored blocks over [0x00 filter byte | row] x h
     std::vector<unsigned char> z;
@@ -71,7 +72,6 @@ bool encode_png(const uint8_t* rgba, int w, int h, std::vector<unsigned char>& o
     chunk(out, "IHDR", ihdr.data(), ihdr.size());
     chunk(out, "IDAT", z.data(), z.size());
     chunk(out, "IEND", nullptr, 0);
-    return true;
 }
 
 }  // namespace
@@ -79,14 +79,17 @@ bool encode_png(const uint8_t* rgba, int w, int h, std::vector<unsigned char>& o
 extern "C" {
 
 int vr_write_png(const char* path, const uint8_t* rgba8_host, int width, int height) {
-    if (!path) return VR_EINVAL;
+    if (!path) return vrb::fail(VR_EINVAL, "null PNG path");
+    if (!rgba8_host) return vrb::fail(VR_EINVAL, "%s: null pixel buffer", path);
+    if (width <= 0 || height <= 0) return vrb::fail(VR_EINVAL, "%s: bad image size %dx%d", path, width, height);
     std::vector<unsigned char> png;
-    if (!encode_png(rgba8_host, width, height, png)) return VR_EINVAL;
+    encode_png(rgba8_host, width, height, png);
     FILE* f = fopen(path, "wb");
-    if (!f) return VR_EINVAL;
+    if (!f) return vrb::fail(VR_EINVAL, "cannot open %s: %s", path, strerror(errno));
     const bool ok = fwrite(png.data(), 1, png.size(), f) == png.size();
+    const int err = errno;
     fclose(f);
-    return ok ? VR_OK : VR_EINVAL;
+    return ok ? VR_OK : vrb::fail(VR_EINVAL, "cannot write %s: %s", path, strerror(err));
 }
 
 }  // extern "C"
@@ -96,8 +99,10 @@ namespace {
 // vr_render_frames_png(_opts): opt_stride as in vr_frames.h
 int render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
                       const char* const* paths, int n_threads) {
-    if (n_views < 0 || (n_views > 0 && (!cams || !paths))) return VR_EINVAL;
+    if (n_views < 0) return vrb::fail(VR_EINVAL, "n_views < 0");
     if (n_views == 0) return VR_OK;
+    if (!cams) return vrb::fail(VR_EINVAL, "null cameras");
+    if (!paths) return vrb::fail(VR_EINVAL, "null PNG paths");
     if (n_threads < 1) n_threads = 1;
     const int w = cams[0].width, h = cams[0].height;
     const size_t frame = (size_t)4 * w * h;
@@ -107,8 +112,9 @@ int render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, c
     std::vector<uint8_t> buf[2];
     buf[0].resize(frame * (size_t)(n_views < slab ? n_views : slab));
     buf[1].resize(buf[0].size());
-    std::atomic<int> failed{0};
-    std::vector<std::thread> workers;
+    // vr_write_png sets the message on its worker thread: the first one is kept for the caller's thread
+    std::mutex err_mu;
+    std::string err;
     auto encode_slab = [&](const uint8_t* base, int v0, int nv) {
         std::atomic<int> next{0};
         std::vector<std::thread> th;
@@ -117,7 +123,10 @@ int render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, c
                 for (;;) {
                     const int i = next.fetch_add(1);
                     if (i >= nv) break;
-                    if (vr_write_png(paths[v0 + i], base + frame * (size_t)i, w, h) != VR_OK) failed.store(1);
+                    if (vr_write_png(paths[v0 + i], base + frame * (size_t)i, w, h) != VR_OK) {
+                        std::lock_guard<std::mutex> lk(err_mu);
+                        if (err.empty()) err = vr_last_error();
+                    }
                 }
             });
         for (auto& x : th) x.join();
@@ -132,10 +141,9 @@ int render_frames_png(const vr_tree* tree, const vr_camera* cams, int n_views, c
         if (pending.joinable()) pending.join();   // previous slab's buffer is free again after this
         pending = std::thread(encode_slab, dst, v0, nv);
         // the next iteration renders into the other buffer while `pending` encodes this one
-        if (k >= 1) { /* buffers alternate; the join above guarantees buf[(k+1)&1] is idle */ }
     }
     if (pending.joinable()) pending.join();
-    return failed.load() ? VR_EINVAL : VR_OK;
+    return err.empty() ? VR_OK : vrb::fail(VR_EINVAL, "%s", err.c_str());
 }
 
 }  // namespace
