@@ -348,7 +348,8 @@ static void sim_park(const ray_t* rays, int W, int H, int theta, int patience, s
 /* ---- MEM mode: DRAM traffic of a work order.  The tiles of all views are handed out in queue order to NW warps (a
  * warp takes the next tile when its current one ends); all busy warps advance one march iteration per round, and every
  * table-word fetch (a 32-byte sector of its table) and every shaded sample's 96-byte record (3 sectors, keyed by its
- * table entry) goes through an LRU model of the L2 in 32-byte sectors.  No associativity, no L1, no cache hints. */
+ * table entry) goes through an LRU model of its SM's L1 (L1KB per SM, 0 = none) and, on a miss, of the L2, both in
+ * 32-byte sectors.  Warp w runs on SM (w / 4) mod NSM.  No associativity, no cache hints. */
 typedef struct {
     uint64_t* key;    /* hash table: key + 1 (0 = empty), linear probing */
     int32_t* slot;
@@ -419,13 +420,25 @@ static inline int lru_touch(lru_t* L, uint64_t k) {   /* 1 on a miss */
     return 1;
 }
 
+/* A work order: the queue items in order, each (view, tx, ty); view -1 = an item with no pixel (past the last view
+   of a view group).  blk = 0: every warp takes the next item of the launch.  blk = n: SM-affine blocks of n items
+   (vr_march.cuh next_item, blk_mode): the warps of one SM take the items of their SM's current block, and the warp
+   that finds it exhausted claims the next block of the launch for its SM. */
 typedef struct {
     const char* name;
     const ray_t* const* vrays;    /* rays of each view */
-    const int32_t* tiles;         /* (view, tx, ty) per queue item */
-    int ntiles, W, H, nw, cap;
-    double tbl_acc, tbl_miss, rec_acc, rec_miss, rounds;
+    int32_t* tiles;               /* (view, tx, ty) per queue item */
+    int ntiles, blk, W, H, nw, nsm, cap, l1cap;
+    double tbl_acc, tbl_l1miss, tbl_miss, rec_acc, rec_l1miss, rec_miss, rounds;
+    double sm_max, sm_min, sm_mean, sm_last, sm_first;   /* per-SM samples; round of each SM's last sample */
 } replay_t;
+
+/* L1 of the SM (when modelled), then L2; returns the DRAM misses and counts the L1 misses */
+static inline int touch2(lru_t* L1, lru_t* L2, uint64_t k, double* l1miss) {
+    if (L1 && !lru_touch(L1, k)) return 0;
+    *l1miss += 1;
+    return lru_touch(L2, k);
+}
 
 static void* replay(void* arg) {
     replay_t* J = (replay_t*)arg;
@@ -433,11 +446,21 @@ static void* replay(void* arg) {
     const uint64_t kRec = 1ull << 40;   /* record sectors: their own address range */
     lru_t L;
     lru_init(&L, J->cap);
+    lru_t* L1 = NULL;
+    if (J->l1cap > 0) {
+        L1 = (lru_t*)malloc((size_t)J->nsm * sizeof(lru_t));
+        for (int s = 0; s < J->nsm; ++s) lru_init(&L1[s], J->l1cap);
+    }
     const ray_t** lane = (const ray_t**)calloc((size_t)J->nw * 32, sizeof(ray_t*));
     uint32_t* pos = (uint32_t*)calloc((size_t)J->nw * 32, 4);
     uint32_t* kp = (uint32_t*)calloc((size_t)J->nw * 32, 4);
     int* alive = (int*)calloc(J->nw, sizeof(int));
     char* busy = (char*)calloc(J->nw, 1);
+    int* sm_blk = (int*)malloc((size_t)J->nsm * sizeof(int));   /* SM's block: next item, end */
+    int* sm_end = (int*)calloc(J->nsm, sizeof(int));
+    double* sm_work = (double*)calloc(J->nsm, sizeof(double));
+    double* sm_last = (double*)calloc(J->nsm, sizeof(double));
+    for (int s = 0; s < J->nsm; ++s) sm_blk[s] = 0;
     int next = 0;
     for (;;) {
         int any = 0;
@@ -445,28 +468,41 @@ static void* replay(void* arg) {
             const ray_t** ln = lane + (size_t)w * 32;
             uint32_t* ps = pos + (size_t)w * 32;
             uint32_t* kq = kp + (size_t)w * 32;
+            const int sm = (w / 4) % J->nsm;   /* 4 warps per CTA, CTAs spread round-robin over the SMs */
             if (!busy[w]) {
-                if (next >= J->ntiles) continue;
-                const int32_t* t = J->tiles + 3 * (size_t)next++;
-                const ray_t* rays = J->vrays[t[0]];
+                int item;
+                if (!J->blk) {
+                    if (next >= J->ntiles) continue;
+                    item = next++;
+                } else {
+                    if (sm_blk[sm] >= sm_end[sm]) {
+                        if (next >= J->ntiles) continue;
+                        sm_blk[sm] = next; sm_end[sm] = next + J->blk; next += J->blk;
+                    }
+                    item = sm_blk[sm]++;
+                }
+                const int32_t* t = J->tiles + 3 * (size_t)item;
                 alive[w] = 0;
+                const ray_t* rays = t[0] >= 0 ? J->vrays[t[0]] : NULL;
                 for (int l = 0; l < 32; ++l) {
                     const int x = t[1] * TW + l % TW, y = t[2] * TH + l / TW;
-                    ln[l] = (x < J->W && y < J->H) ? &rays[(size_t)y * J->W + x] : NULL;
+                    ln[l] = (rays && x < J->W && y < J->H) ? &rays[(size_t)y * J->W + x] : NULL;
                     ps[l] = 0;
                     if (ln[l]) { kq[l] = ln[l]->koff; if (ln[l]->n) ++alive[w]; }
                 }
                 busy[w] = 1;
             }
             any = 1;
+            lru_t* l1 = L1 ? &L1[sm] : NULL;
             for (int l = 0; l < 32; ++l) {
                 if (!ln[l] || ps[l] >= ln[l]->n) continue;
                 const uint8_t v = g_trace[ln[l]->off + ps[l]++];
-                for (int f = v & 15; f > 0; --f) { J->tbl_acc += 1; J->tbl_miss += lru_touch(&L, g_keys[kq[l]++]); }
+                sm_work[sm] += 1; sm_last[sm] = J->rounds;
+                for (int f = v & 15; f > 0; --f) { J->tbl_acc += 1; J->tbl_miss += touch2(l1, &L, g_keys[kq[l]++], &J->tbl_l1miss); }
                 if (v & 128) {
                     const uint64_t r = (uint64_t)g_keys[kq[l]++] * 3;
                     J->rec_acc += 1;
-                    for (int s = 0; s < 3; ++s) J->rec_miss += lru_touch(&L, kRec + r + s);
+                    for (int s = 0; s < 3; ++s) J->rec_miss += touch2(l1, &L, kRec + r + s, &J->rec_l1miss);
                 }
                 if (ps[l] >= ln[l]->n) --alive[w];
             }
@@ -475,7 +511,16 @@ static void* replay(void* arg) {
         if (!any) break;
         J->rounds += 1;
     }
-    free(lane); free(pos); free(kp); free(alive); free(busy);
+    J->sm_max = J->sm_min = sm_work[0]; J->sm_last = J->sm_first = sm_last[0]; J->sm_mean = 0;
+    for (int s = 0; s < J->nsm; ++s) {
+        J->sm_mean += sm_work[s] / J->nsm;
+        if (sm_work[s] > J->sm_max) J->sm_max = sm_work[s];
+        if (sm_work[s] < J->sm_min) J->sm_min = sm_work[s];
+        if (sm_last[s] > J->sm_last) J->sm_last = sm_last[s];
+        if (sm_last[s] < J->sm_first) J->sm_first = sm_last[s];
+    }
+    free(lane); free(pos); free(kp); free(alive); free(busy); free(sm_blk); free(sm_end); free(sm_work); free(sm_last);
+    if (L1) { for (int s = 0; s < J->nsm; ++s) lru_free(&L1[s]); free(L1); }
     lru_free(&L);
     return NULL;
 }
@@ -503,10 +548,84 @@ static int32_t* make_order(int ncam, int ntx, int nty, int group) {
     return t;
 }
 
+/* SM-affine blocks of bw x bh tiles of g consecutive views at the same position, in the order (block row, view group,
+   block x) (vr_march.cuh decode_item, blk_mode); inside a block the view is innermost (view_inner) or the tile is.
+   Every block has bw * bh * g items; those past the image edge or the last view have no pixel.  *n = items. */
+static int32_t* make_blocks(int ncam, int ntx, int nty, int bw, int bh, int g, int view_inner, int* n) {
+    const int bx = (ntx + bw - 1) / bw, by = (nty + bh - 1) / bh, ng = (ncam + g - 1) / g, nbt = bw * bh * g;
+    *n = bx * by * ng * nbt;
+    int32_t* t = (int32_t*)malloc((size_t)*n * 3 * 4);
+    size_t k = 0;
+    for (int r = 0; r < by; ++r)
+        for (int gi = 0; gi < ng; ++gi)
+            for (int x = 0; x < bx; ++x)
+                for (int i = 0; i < nbt; ++i) {
+                    const int v = view_inner ? i % g : i / (bw * bh), tl = view_inner ? i / g : i % (bw * bh);
+                    const int view = gi * g + v;
+                    t[k++] = view < ncam ? view : -1; t[k++] = x * bw + tl % bw; t[k++] = r * bh + tl / bw;
+                }
+    return t;
+}
+
+/* every (view, tile) exactly once */
+static int check_order(const int32_t* t, int n, int ncam, int ntx, int nty) {
+    char* seen = (char*)calloc((size_t)ncam * ntx * nty, 1);
+    int bad = 0;
+    for (int i = 0; i < n; ++i) {
+        const int v = t[3 * i], x = t[3 * i + 1], y = t[3 * i + 2];
+        if (v < 0 || x >= ntx || y >= nty) continue;
+        if (seen[((size_t)v * nty + y) * ntx + x]++) bad = 1;
+    }
+    for (size_t i = 0; i < (size_t)ncam * ntx * nty; ++i) if (seen[i] != 1) bad = 1;
+    free(seen);
+    return bad;
+}
+
+typedef struct { const char* name; int group, bw, bh, g, view_inner; } order_t;
+static const order_t g_orders[] = {
+    {"view-major (before 3c9fce8)", 0, 0, 0, 0, 0},
+    {"rows across all views (current)", -1, 0, 0, 0, 0},
+    {"blocks 8x8 tiles x 1 view", 0, 8, 8, 1, 0},
+    {"blocks 4x4 tiles x 1 view", 0, 4, 4, 1, 0},
+    {"blocks 16x8 tiles x 1 view", 0, 16, 8, 1, 0},
+    {"blocks 8x8 x 2 views, view inner", 0, 8, 8, 2, 1},
+    {"blocks 8x8 x 2 views, tile inner", 0, 8, 8, 2, 0},
+    {"blocks 8x8 x 4 views, view inner", 0, 8, 8, 4, 1},
+    {"blocks 8x8 x 4 views, tile inner", 0, 8, 8, 4, 0},
+    {"blocks 8x8 x 8 views, view inner", 0, 8, 8, 8, 1},
+    {"blocks 8x8 x 8 views, tile inner", 0, 8, 8, 8, 0},
+    {"blocks 4x4 x 4 views, view inner", 0, 4, 4, 4, 1},
+    {"blocks 4x4 x 4 views, tile inner", 0, 4, 4, 4, 0},
+    {"blocks 4x2 x 8 views, view inner", 0, 4, 2, 8, 1},
+};
+enum { kOrders = sizeof(g_orders) / sizeof(g_orders[0]) };
+
+/* lane_sim --check-orders <views> <W> <H>: checks that every order of the MEM replay visits every (view, tile)
+   exactly once; exit status 1 if one does not */
+static int check_orders(int ncam, int W, int H) {
+    const int ntx = (W + 3) / 4, nty = (H + 7) / 8;
+    int bad = 0;
+    for (int k = 0; k < kOrders; ++k) {
+        const order_t* o = &g_orders[k];
+        int n = ncam * ntx * nty;
+        int32_t* t = o->bw ? make_blocks(ncam, ntx, nty, o->bw, o->bh, o->g, o->view_inner, &n)
+                           : make_order(ncam, ntx, nty, o->group < 0 ? ncam : o->group);
+        const int b = check_order(t, n, ncam, ntx, nty);
+        printf("%-36s %s\n", o->name, b ? "BAD" : "ok");
+        bad |= b;
+        free(t);
+    }
+    return bad;
+}
+
 static void mem_main(const orc_tree* tree, const orc_camera* cams, int ncam, int W, int H) {
     const int nw = getenv("NWARPS") ? atoi(getenv("NWARPS")) : 4224;   /* 8 CTAs x 4 warps x 132 SMs */
+    const int nsm = getenv("NSM") ? atoi(getenv("NSM")) : 132;
     const double l2mb = getenv("L2MB") ? atof(getenv("L2MB")) : 50.0;
-    const int cap = (int)(l2mb * 1024 * 1024 / 32);
+    /* L1 per SM: 256 KB less the 100 KB shared-memory carve-out that 8 CTAs x (9.2 KB + 1 KB reserved) need */
+    const double l1kb = getenv("L1KB") ? atof(getenv("L1KB")) : 156.0;
+    const int cap = (int)(l2mb * 1024 * 1024 / 32), l1cap = (int)(l1kb * 1024 / 32);
+    const int ntx = (W + 3) / 4, nty = (H + 7) / 8;
     orc_options opt;
     orc_default_options(&opt);
     ray_t** vrays = (ray_t**)malloc((size_t)ncam * sizeof(ray_t*));
@@ -520,24 +639,36 @@ static void mem_main(const orc_tree* tree, const orc_camera* cams, int ncam, int
     }
     printf("MEM: %d views %dx%d, %d warps in flight, L2 %.0f MB (%d sectors); %.2fM samples, %.3fM shaded per view\n",
            ncam, W, H, nw, l2mb, cap, g_trace_n / 1e6 / ncam, nshade / 1e6 / ncam);
-    const int ntx = (W + 3) / 4, nty = (H + 7) / 8;
-    const int groups[5] = {0, ncam, 4, 8, 16};
-    const char* names[5] = {"view-major (parent)", "rows outermost, all views", "rows outermost, groups of 4",
-                            "rows outermost, groups of 8", "rows outermost, groups of 16"};
-    replay_t J[5];
-    pthread_t th[5];
-    for (int k = 0; k < 5; ++k) {
+    printf("L1 per SM %.0f KB (%d sectors, 0 = no L1 model), %d SMs, warp w on SM (w / 4) mod %d\n", l1kb, l1cap, nsm, nsm);
+    replay_t J[kOrders];
+    pthread_t th[kOrders];
+    for (int k = 0; k < kOrders; ++k) {
+        const order_t* o = &g_orders[k];
         memset(&J[k], 0, sizeof(J[k]));
-        J[k].name = names[k]; J[k].vrays = (const ray_t* const*)vrays; J[k].tiles = make_order(ncam, ntx, nty, groups[k]);
-        J[k].ntiles = ncam * ntx * nty; J[k].W = W; J[k].H = H; J[k].nw = nw; J[k].cap = cap;
+        J[k].name = o->name; J[k].vrays = (const ray_t* const*)vrays;
+        J[k].ntiles = ncam * ntx * nty;
+        if (o->bw) {
+            J[k].tiles = make_blocks(ncam, ntx, nty, o->bw, o->bh, o->g, o->view_inner, &J[k].ntiles);
+            J[k].blk = o->bw * o->bh * o->g;
+        } else {
+            J[k].tiles = make_order(ncam, ntx, nty, o->group < 0 ? ncam : o->group);
+        }
+        J[k].W = W; J[k].H = H; J[k].nw = nw; J[k].nsm = nsm; J[k].cap = cap; J[k].l1cap = l1cap;
         pthread_create(&th[k], NULL, replay, &J[k]);
     }
-    printf("%-30s %14s %14s %14s %12s %12s\n", "order", "tables MB/fr", "records MB/fr", "DRAM MB/fr", "tbl L2 hit", "rec L2 hit");
-    for (int k = 0; k < 5; ++k) {
+    /* hit rates per access (tables: one 32-byte sector, records: 3 sectors); "rec L2 hit" is of the L1 misses;
+       SM samples: most / fewest per SM over the mean; tail: rounds between the first and the last SM running dry,
+       over all rounds of the launch */
+    printf("%-36s %8s %8s %8s %10s %10s %9s %9s %6s\n", "order", "tbl L1", "rec L1", "rec L2", "tbl MB/fr",
+           "DRAM MB/fr", "SM max", "SM min", "tail");
+    for (int k = 0; k < kOrders; ++k) {
         pthread_join(th[k], NULL);
         const double tb = J[k].tbl_miss * 32 / 1e6 / ncam, rb = J[k].rec_miss * 32 / 1e6 / ncam;
-        printf("%-30s %14.1f %14.1f %14.1f %11.1f%% %11.1f%%\n", J[k].name, tb, rb, tb + rb,
-               100 * (1 - J[k].tbl_miss / (J[k].tbl_acc + 1e-9)), 100 * (1 - J[k].rec_miss / (3 * J[k].rec_acc + 1e-9)));
+        printf("%-36s %7.1f%% %7.1f%% %7.1f%% %10.1f %10.1f %9.3f %9.3f %5.1f%%\n", J[k].name,
+               100 * (1 - J[k].tbl_l1miss / (J[k].tbl_acc + 1e-9)), 100 * (1 - J[k].rec_l1miss / (3 * J[k].rec_acc + 1e-9)),
+               100 * (1 - J[k].rec_miss / (J[k].rec_l1miss + 1e-9)), tb, tb + rb, J[k].sm_max / J[k].sm_mean,
+               J[k].sm_min / J[k].sm_mean, 100 * (J[k].sm_last - J[k].sm_first) / (J[k].rounds + 1e-9));
+        free(J[k].tiles);
     }
 }
 
@@ -549,7 +680,8 @@ static void report(const char* name, const stats_t* S, int frames) {
 }
 
 int main(int argc, char** argv) {
-    if (argc < 2) { fprintf(stderr, "usage: lane_sim dump.bin\n"); return 2; }
+    if (argc == 5 && !strcmp(argv[1], "--check-orders")) return check_orders(atoi(argv[2]), atoi(argv[3]), atoi(argv[4]));
+    if (argc < 2) { fprintf(stderr, "usage: lane_sim dump.bin | lane_sim --check-orders views W H\n"); return 2; }
     FILE* f = fopen(argv[1], "rb");
     if (!f) { perror("open"); return 1; }
     int64_t hdr[4];  /* capacity, W, H, n_cams */

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Design tool: dump the bench tree's topology + sigma and a few poses, build tools/lane_sim.c and run
 it.  Ranks lane-scheduling policies of the march kernel on the CPU (no GPU needed).
-MEM=1 replays the DRAM traffic of the batch work orders instead (give it consecutive orbit poses:
-MEM=1 VIEWS=40-71)."""
+MEM=1 replays the memory traffic of the batch work orders instead -- per-SM L1 (L1KB, default 156) and L2 (L2MB,
+default 50) hit rates, DRAM bytes and the per-SM balance of the plain and the SM-affine block orders (give it
+consecutive orbit poses: MEM=1 VIEWS=40-55)."""
 import os
 import subprocess
 import sys

@@ -53,20 +53,27 @@ void set_work(LaunchDev& P, const LaunchCfg& cfg, bool blocks = true) {
     P.tiles_x = (P.w + kTW - 1) / kTW;
     P.tiles_y = (P.h + kTH - 1) / kTH;
     P.work_counter = cfg.queue;
-    // Batches can have the queue hand out blocks of 8x8 tiles, the warps of an SM sharing a block (vr_march.cuh next_item).
-    // Measured: a gain on config 4 (SH25, 160-byte records, 1080p; still +5 % over single tiles in the rows-across-views
-    // order), none on config 2 (SH16): on for 25 basis functions only.  It needs enough blocks
-    // per SM to balance (a block is ~20 us of an SM), so single frames always keep one tile per item.
-    const long long bx = (P.tiles_x + kBlkW - 1) / kBlkW, by = (P.tiles_y + kBlkH - 1) / kBlkH, nb = bx * by * P.n_views;
-    const bool want = P.tree.kbd == 25 && P.n_views >= 2 && nb >= 16LL * cfg.num_sms;
+    // Batches have the queue hand out blocks of 64 tiles, the warps of an SM sharing a block (vr_march.cuh next_item).
+    // Up to 16 basis functions: 4x4 tiles of 4 consecutive views, view innermost, so that the colour records
+    // neighbouring poses share are read from the SM's L1 instead of from L2 (DESIGN.md 4: modelled record L1 hit rate
+    // 7 % -> 43 %; config 2 +0.2 to +4.8 % over three H100 sessions).  25 basis functions (160-byte records,
+    // config 4): 8x8 tiles of one view, which measured 1-2 % faster there than the 4-view blocks.  A block needs
+    // enough blocks per SM to balance (a block is ~20 us of an SM), so single frames and small batches keep one tile
+    // per item.
+    const int gs = P.tree.kbd == 25 ? 0 : 2, ws = P.tree.kbd == 25 ? 3 : 2;
+    const int G = 1 << gs, bw = 1 << ws, bh = kBlkTiles / (G * bw);
+    const long long bx = (P.tiles_x + bw - 1) / bw, by = (P.tiles_y + bh - 1) / bh, ng = (P.n_views + G - 1) / G;
+    const long long nb = bx * by * ng;
+    const bool want = P.n_views >= G && P.n_views >= 2 && nb >= 16LL * cfg.num_sms;
     if (blocks && want && nb * kBlkTiles <= 0x7fffffffLL) {
         P.blk_mode = 1; P.blocks_x = (int)bx; P.n_blocks = (int)nb;
-        P.n_tiles = (int)(nb * kBlkTiles);   // item ids (block * 64 + tile), incl. the tiles beyond the image edge
-        set_div((uint32_t)bx, P.div_row_mul, P.div_row_shift);   // block -> (block row, view) pair
-        set_div((uint32_t)P.n_views, P.div_view_mul, P.div_view_shift);
+        P.blk_gshift = gs; P.blk_wshift = ws; P.blk_groups = (int)ng;
+        P.n_tiles = (int)(nb * kBlkTiles);   // item ids (block * 64 + index), incl. the tiles beyond the image edge
+        set_div((uint32_t)bx, P.div_row_mul, P.div_row_shift);   // block -> (block row, view group) pair
+        set_div((uint32_t)ng, P.div_view_mul, P.div_view_shift);
         return;
     }
-    P.blk_mode = 0; P.blocks_x = 0; P.n_blocks = 0;
+    P.blk_mode = 0; P.blocks_x = 0; P.n_blocks = 0; P.blk_gshift = 0; P.blk_wshift = 0; P.blk_groups = 0;
     P.n_tiles = P.tiles_x * P.tiles_y * P.n_views;
     set_div((uint32_t)P.tiles_x, P.div_row_mul, P.div_row_shift);    // item -> (tile row, view) pair (decode_item)
     set_div((uint32_t)P.n_views, P.div_view_mul, P.div_view_shift);

@@ -90,13 +90,7 @@ inline void set_div(uint32_t d, uint32_t& mul, int32_t& shift) {
 
 // Work queue of the persistent kernels.  One slot per launch in flight: {head, done CTAs}, then per SM id (mod 256) a
 // 64-bit block state and a 32-bit lock (SM-local tile blocks, vr_march.cuh next_item).
-#ifndef VR_BLK_W
-#define VR_BLK_W 8
-#endif
-#ifndef VR_BLK_H
-#define VR_BLK_H 8
-#endif
-constexpr int kBlkW = VR_BLK_W, kBlkH = VR_BLK_H, kBlkTiles = kBlkW * kBlkH;    // a block = 8x8 warp tiles = 32x64 pixels
+constexpr int kBlkShift = 6, kBlkTiles = 1 << kBlkShift;   // a block = 64 warp tiles: views x tiles wide x tiles high
 constexpr uint32_t kBlkDone = 0xfffffffdu, kBlkInvalid = 0xffffffffu;
 constexpr unsigned long long kBlkIdle = 0x80000000ull;             // low word of a state that holds no tiles
 constexpr int kQueueSlotBytes = 4096, kQueueStateOff = 64, kQueueLockOff = 64 + 256 * 8;
@@ -122,10 +116,11 @@ struct LaunchDev {
     uint32_t div_view_mul, div_row_mul;
     int32_t div_view_shift, div_row_shift;
     unsigned int* work_counter;         // persistent kernels: global work queue {head, done CTAs} (start of a queue slot)
-    // SM-local tile blocks (batches, vr_march.cuh next_item): the queue hands out BLOCKS of 8x8 warp tiles, the warps of
-    // one SM share a block, so that neighbouring tiles -- same tables, same records -- are marched at the same time on
-    // the same L1.  blk_mode 0: one tile per queue item (single frames: finest balance).
-    int32_t blk_mode, blocks_x, n_blocks;
+    // SM-local tile blocks (batches, vr_march.cuh next_item): the queue hands out BLOCKS of 64 warp tiles -- the same
+    // 2^blk_wshift x 2^(6 - blk_gshift - blk_wshift) tiles of 2^blk_gshift consecutive views --, the warps of one SM
+    // share a block, so that neighbouring tiles of neighbouring poses -- same tables, same records -- are marched at the
+    // same time on the same L1.  blk_mode 0: one tile per queue item (single frames: finest balance).
+    int32_t blk_mode, blocks_x, n_blocks, blk_gshift, blk_wshift, blk_groups;   // blk_groups: view groups of the batch
     unsigned char* pool;                // ray-pool kernels: parked-ray stacks, one per CTA (vr_march_q.cuh); nullptr = no parking
     unsigned long long* trace;          // diagnostics: per work item {start ns, end ns, smid, warp}
     // per-view options (vr_render_batch_opts): device array of n_views entries, read only by the kOutViewOpts
