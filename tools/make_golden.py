@@ -17,6 +17,8 @@ built from the reference sources by oracle/Makefile.ref).  Needs a GPU.
   python tools/make_golden.py --query OUT        tests/golden/ref/query_*.npz, the reference's query_single_from_root
                                                  (oracle/_ref/libref_query.so) on the trees and point sets of
                                                  tests/query_cases.py
+  python tools/make_golden.py --edge OUT         tests/golden/ref/edge_*.npz, launch_renderer (float RGBA and bytes) of
+                                                 the trees, views and options of tests/edge_cases.py
 
 OUT receives the files; copy them to tests/golden/ (or tests/golden/ref/) and commit them.
 """
@@ -169,6 +171,28 @@ def queries(out_dir, only, tmpdir):
         print(name, "points", len(pts), "data_dim", data.shape[1], "max cube", float(cube.max()), flush=True)
 
 
+def edge_frames(out_dir, only, tmpdir):
+    import edge_cases as ec
+    for name in ec.TREES:
+        if only and name not in only:
+            continue
+        st, npz = ec.edge_tree(name)
+        path = os.path.join(tmpdir, name + ".npz")
+        ec.write_tree_file(name, st, npz, path)
+        rt = rb.RefTree(path)
+        assert bool(rt.info()["use_ndc"]) == (name in ec.NDC)
+        for fr in ec.frames_of(name):
+            _, W, H, fx, fy, pose, kw, comp = ec.frame(fr, st)
+            c12 = synth.c2w_to_colmajor12(pose)
+            rin, din = comp if comp is not None else (None, None)
+            f = rt.render_f32(W, H, fx, fy, c12, rb.make_options(**kw), rgba_in=rin, depth_in=din)
+            u = rt.render_u8(W, H, fx, fy, c12, rb.make_options(**kw), rgba_in=rin, depth_in=din)
+            np.savez_compressed(os.path.join(out_dir, os.path.basename(ec.golden_path(fr))), **ec.record(fr, f, u))
+            print(fr, f"{W}x{H}", "alpha mean %.3f" % f[..., 3].mean(), "rgb mean %.3f" % f[..., :3].mean(), flush=True)
+        rt.close()
+        os.remove(path)
+
+
 def main():
     args = sys.argv[1:]
     if "--query" in args:
@@ -195,7 +219,8 @@ def main():
     frames = "--frames" in args
     wire = "--wire" in args
     probe = "--probe" in args
-    args = [a for a in args if a not in ("--frames", "--wire", "--probe")]
+    edge = "--edge" in args
+    args = [a for a in args if a not in ("--frames", "--wire", "--probe", "--edge")]
     if not args:
         raise SystemExit(__doc__)
     if not rb.available() or (wire and not ref_wire.available()) or (probe and not probe_oracle.ref_available()):
@@ -204,7 +229,8 @@ def main():
     out_dir, only = args[0], args[1:]
     os.makedirs(out_dir, exist_ok=True)
     with tempfile.TemporaryDirectory() as tmpdir:
-        run = wireframes if wire else probe_frames if probe else reference_frames if frames else golden_cases
+        run = (wireframes if wire else probe_frames if probe else reference_frames if frames else edge_frames if edge
+               else golden_cases)
         run(out_dir, only, tmpdir)
 
 

@@ -152,14 +152,18 @@ class SynthTree:
     def nbytes(self) -> int:
         return self.child.nbytes + self.data.nbytes
 
-    def save_npz(self, path: str) -> None:
-        """Write the App. C schema; readable by the unchanged loader (n3tree.cpp:228-362)."""
+    def npz_dict(self) -> dict:
+        """The arrays of the App. C schema, as ``np.load`` of the saved file returns them."""
         kw = dict(data_dim=np.int64(self.data_dim), data_format=np.array(self.data_format),
                   invradius3=self.invradius3.astype(np.float32), offset=self.offset.astype(np.float32),
                   child=self.child, data=self.data)
         if self.extra is not None:
             kw["extra_data"] = self.extra.astype(np.float32)
-        np.savez(path, **kw)
+        return kw
+
+    def save_npz(self, path: str) -> None:
+        """Write the App. C schema; readable by the unchanged loader (n3tree.cpp:228-362)."""
+        np.savez(path, **self.npz_dict())
 
 
 def _hash_u01(ix, iy, iz, salt):
