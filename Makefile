@@ -2,8 +2,6 @@
 #   make lib      volrend_b200/libvolrend_b200.so   the product: C-ABI + sm_90a kernels
 #   make oracle   oracle/liboracle.so               CPU restatement (test infrastructure), and
 #                 oracle/libprobe_oracle.so         the same with the probe disc
-#   make exp      volrend_b200/libvolrend_b200_exp.so  the same library with the measured experiment kernels
-#                                                   (-DVR_EXPERIMENTS; the parity tests check them)
 #   make ref      oracle/_ref/*                     the unmodified reference (+ its gen_wireframe, probe and mesh harnesses), built from
 #                                                   $(VOLREND_REF) (only when it exists)
 #   make shim     oracle/_ref/volrend_headless ...  reference CLI linked against OUR backend
@@ -13,26 +11,16 @@ CC        ?= gcc
 ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Iinclude -Ivolrend_b200/csrc \
              -diag-suppress 20012
-# tuning builds: make lib VR_BLOCK=128 VR_MINB=7 SUFFIX=_b128m7  (selected at run time with VR_LIB_SUFFIX)
-VR_BLOCK  ?= 128
-VR_MINB   ?= 8
-SUFFIX    ?=
-VR_TW     ?= 4
-EXTRA     ?=
-NVFLAGS   += -DVR_BLOCK=$(VR_BLOCK) -DVR_MINB=$(VR_MINB) -DVR_TW=$(VR_TW) $(EXTRA)
-OBJ       := build/obj$(SUFFIX)
+OBJ       := build/obj
 KBDS      := m1 1 4 9 16 25
 KOBJS     := $(foreach k,$(KBDS),$(OBJ)/vr_kernels_$(k).o)
-LIB       := volrend_b200/libvolrend_b200$(SUFFIX).so
+LIB       := volrend_b200/libvolrend_b200.so
 VOLREND_REF ?= /root/reference
 
-.PHONY: all lib exp oracle ref shim clean
+.PHONY: all lib oracle ref shim clean
 all: lib oracle
 
 lib: $(LIB)
-
-exp:
-	$(MAKE) lib SUFFIX=_exp EXTRA=-DVR_EXPERIMENTS
 
 $(OBJ)/vr_kernels_m1.o: volrend_b200/csrc/vr_kernels_inst.cu volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_march_q.cuh volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
@@ -100,4 +88,4 @@ shim:
 	 else echo "reference tree $(VOLREND_REF) not present: shim needs the reference headers"; fi
 
 clean:
-	rm -rf build $(LIB) volrend_b200/libvolrend_b200_exp.so oracle/liboracle.so oracle/_ref
+	rm -rf build $(LIB) oracle/liboracle.so oracle/_ref

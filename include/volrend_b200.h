@@ -100,10 +100,11 @@ typedef struct {
     int64_t capacity;
     int32_t max_depth;               /* deepest leaf (root children = 1) */
     int32_t rec_bytes;               /* padded leaf-record stride */
-    int64_t node_bytes, rec_total_bytes, top_bytes; /* slot-indexed layout (resident in -DVR_EXPERIMENTS builds only) */
+    int64_t node_bytes, rec_total_bytes, top_bytes; /* sizes of the slot-indexed layout (node words, records,
+                                                       a 16^3 top grid); never resident */
     int32_t kernel_basis;            /* -1 RGBA, 1, 4, 9, 16, 25 */
     int32_t wide_parity;             /* v: internal nodes of depth d with (d + v) % 2 == 0 own a 64-entry table (+ the root);
-                                        the v with fewer tables is chosen per tree (% 3 and 512 entries in VR_WIDE_LV=3 builds) */
+                                        the v with fewer tables is chosen per tree */
     int64_t n_tables;
     int64_t wide_bytes, wrecs_bytes; /* 64-entry tables; colour records indexed by table entry */
     int64_t kernel_bytes;            /* what the march kernels can touch: wide_bytes + wrecs_bytes */

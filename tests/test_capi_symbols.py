@@ -32,6 +32,8 @@ def test_version_and_variant(built):
     l = lib()
     assert b"sm_90a" in l.vr_version()
     assert l.vr_set_variant(9) != 0 and b"variant" in l.vr_last_error()
+    for v in (8, 1, 2, 3, 4, 5, 6, 19, 3 + 16 * 64, 3 + 16 * 65):   # no kernel behind these ids
+        assert l.vr_set_variant(v) != 0, v
     assert l.vr_set_variant(300) != 0
     assert l.vr_set_variant(-1) != 0
     assert l.vr_set_variant(0) == 0 and l.vr_get_variant() == 0

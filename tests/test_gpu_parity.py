@@ -7,9 +7,7 @@ positions are bit-identical, so we also assert the exact work counters and that 
 bit-identical to the reference kernel."""
 import ctypes as C
 import os
-import pickle
 import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -18,10 +16,8 @@ from conftest import ROOT
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
-QUEUE, INLINE, POOL = 7, 3 + 16 * 193, 8     # the product kernels (vr_kernels.h): shading queue, inline shading, queue + ray pool
-# round-1 experiment kernels: present only in the -DVR_EXPERIMENTS build (make exp: libvolrend_b200_exp.so)
-VARIANTS = [QUEUE, POOL, INLINE, 1, 2, 3, 4, 5, 6, 19, 3 + 16 * 64, 3 + 16 * 65]
-EXP_SUFFIX = "_exp"
+QUEUE, INLINE = 7, 3 + 16 * 193     # the two kernels (vr_kernels.h): shading queue, inline shading
+VARIANTS = [QUEUE, INLINE]
 TREE_NAMES = ["sh1_full4", "sh16_d6", "sh9_d6", "sh4_d5", "sh25_d5", "rgba_d5", "sg9_d5", "asg4_d5", "sg7_d5"]
 
 
@@ -76,12 +72,6 @@ def dev_trees(small_trees):
     return {k: (st, N3Tree.from_synth(st)) for k, st in small_trees.items()}
 
 
-def in_product_library(variant) -> bool:
-    """Whether the product library has the variant for some basis size (else it is an experiment kernel)."""
-    from volrend_b200 import lib
-    return any(lib().vr_variant_supported(kbd, variant) for kbd in (-1, 1, 4, 9, 16, 25))
-
-
 def all_formats_case(name):
     from volrend_b200 import synth
     pose = synth.config1_pose() if name == "sh1_full4" else synth.nerf_synthetic_test_poses(8)[(len(name) * 3) % 8]
@@ -95,42 +85,21 @@ def render_or_refusal(tree, cam, variant):
     if rc != 0:                    # not in this library at all: never render the default in its place
         return rc
     try:
-        return gpu_render(tree, cam, RenderOptions(), variant=variant, counters=(variant in (QUEUE, POOL, INLINE, 5, 6)))   # instrumented builds of the two product kernels
+        return gpu_render(tree, cam, RenderOptions(), variant=variant, counters=True)
     except VolrendError as e:
         return e.code
     finally:
         lib().vr_set_variant(0)
 
 
-@pytest.fixture(scope="module")
-def experiment_renders(built, small_trees, tmp_path_factory):
-    """The renders of test_matches_oracle_all_formats for the variants that only the experiments build
-    (libvolrend_b200_exp.so) has, made by that library in a process of its own."""
-    from volrend_b200 import _capi
-    exp_lib = _capi.LIB_PATH[:-len(".so")] + EXP_SUFFIX + ".so"
-    assert os.path.exists(exp_lib), f"{exp_lib} is missing: __graft_entry__.build() (make exp) builds it"
-    d = tmp_path_factory.mktemp("experiments")
-    with open(d / "trees.pkl", "wb") as fh:
-        pickle.dump({n: small_trees[n] for n in TREE_NAMES}, fh)
-    variants = [v for v in VARIANTS if not in_product_library(v)]
-    env = dict(os.environ, VR_LIB_SUFFIX=EXP_SUFFIX)
-    subprocess.run([sys.executable, __file__, str(d / "trees.pkl"), ",".join(map(str, variants)), str(d / "out.pkl")],
-                   env=env, cwd=ROOT, check=True, timeout=900)
-    with open(d / "out.pkl", "rb") as fh:
-        return pickle.load(fh)
-
-
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("name", TREE_NAMES)
-def test_matches_oracle_all_formats(built, dev_trees, request, name, variant):
+def test_matches_oracle_all_formats(built, dev_trees, name, variant):
     from volrend_b200 import _capi, lib
     st, tree = dev_trees[name]
     cam, _ = all_formats_case(name)
-    if in_product_library(variant):
-        got = render_or_refusal(tree, cam, variant)
-        assert isinstance(got, int) != supported(tree, variant)
-    else:
-        got = request.getfixturevalue("experiment_renders")[(name, variant)]
+    got = render_or_refusal(tree, cam, variant)
+    assert isinstance(got, int) != supported(tree, variant)
     if isinstance(got, int):       # no kernel of this variant for this basis size: refused, never a fall-back
         assert got == _capi.VR_EUNSUPPORTED, got
         assert lib().vr_get_variant() == 0
@@ -243,7 +212,7 @@ def test_tiles_batches_and_variants_are_bit_identical(built, dev_trees):
         x0, y0, w, h = tile
         assert np.array_equal(ft, full[1][0][y0:y0 + h, x0:x0 + w]), tile
         assert np.array_equal(ut, full[1][1][y0:y0 + h, x0:x0 + w]), tile
-    for v in (QUEUE, POOL, INLINE, 1, 5):
+    for v in VARIANTS:
         if not supported(tree, v):
             continue
         lib().vr_set_variant(v)
@@ -353,9 +322,7 @@ def test_full_size_properties(built):
     cams = [make_cam(800, 800, p) for p in poses]
     opt = RenderOptions()
     outs = {}
-    for v in (QUEUE, INLINE, POOL):
-        if not supported(tree, v):
-            continue
+    for v in VARIANTS:
         lib().vr_set_variant(v)
         imgs = torch.zeros((len(cams), 800, 800, 4), dtype=torch.uint8, device="cuda")
         fo = torch.zeros((len(cams), 800, 800, 4), dtype=torch.float32, device="cuda")
@@ -368,9 +335,6 @@ def test_full_size_properties(built):
     f, u, cnt = outs[QUEUE]
     assert np.array_equal(f, outs[INLINE][0]) and np.array_equal(u, outs[INLINE][1])     # variant-independent
     assert cnt == outs[INLINE][2]
-    # the ray pool moves rays between warps, never changes what a ray computes
-    if POOL in outs:
-        assert np.array_equal(f, outs[POOL][0]) and np.array_equal(u, outs[POOL][1]) and cnt == outs[POOL][2]
     assert np.isfinite(f).all() and f[..., 3].min() >= 0 and f[..., 3].max() <= 1
     assert (f[..., :3] >= 0).all() and (f[..., :3] <= 1 + 1e-5).all()         # sigmoid colours, bg <= 1
     assert np.all(u[..., 3] == 255)
@@ -603,16 +567,3 @@ def test_headless_mg_cli(built, small_trees, tmp_path):
             _, u, _ = gpu_render(tree, make_cam(96, 68, poses[i]), RenderOptions())
             assert np.array_equal(got, u)
 
-
-if __name__ == "__main__":
-    # experiment_renders: python test_gpu_parity.py <trees.pkl> <variant,...> <out.pkl>, run with VR_LIB_SUFFIX=_exp
-    from volrend_b200 import N3Tree
-    with open(sys.argv[1], "rb") as fh:
-        synth_trees = pickle.load(fh)
-    out = {}
-    for tree_name, synth_tree in synth_trees.items():
-        device_tree = N3Tree.from_synth(synth_tree)
-        for v in map(int, sys.argv[2].split(",")):
-            out[(tree_name, v)] = render_or_refusal(device_tree, all_formats_case(tree_name)[0], v)
-    with open(sys.argv[3], "wb") as fh:
-        pickle.dump(out, fh)

@@ -16,7 +16,7 @@ from volrend_b200 import synth, N3Tree, Camera, RenderOptions, launch_renderer, 
 from oracle import binding as ob  # noqa: E402
 from oracle import ref_binding as rb  # noqa: E402
 
-VARIANTS = [int(v) for v in os.environ.get("VR_VARIANTS", "1,3,5,6").split(",")]
+VARIANTS = [int(v) for v in os.environ.get("VR_VARIANTS", "7,3091").split(",")]
 out = {}
 os.makedirs("gpurun_out", exist_ok=True)
 dev = torch.device("cuda:0")

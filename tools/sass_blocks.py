@@ -2,9 +2,9 @@
 """Instruction counts of the hot blocks of the batch march kernel, read from its SASS (no GPU needed).
 
 Compiles volrend_b200/csrc/vr_kernels_inst.cu for sm_90a to a cubin (one per basis size), disassembles the product
-batch kernel march_persistent_kernel<KBD, false, false, kOutLinear, 193> with cuobjdump and splits its march loop:
+batch kernel march_persistent_kernel<KBD, false, kOutLinear> with cuobjdump and splits its march loop:
 
-  march loop   the innermost loop that contains the colour-record loads (LDG.E.NA.128)
+  march loop   the innermost loop that contains the colour-record loads (LDG.E.128.CONSTANT)
   fetch loop   the loop nested in it: one more table fetch of find_leaf_wide
   shading      the forward branch of the march loop that skips the record loads (sigma > sigma_thresh): the
                expf / weight, the record fetch and the colour of one shaded sample.  "common" leaves out the
@@ -39,9 +39,12 @@ def nvcc_path():
     sys.exit("nvcc not found (set CUDA_HOME or put nvcc on PATH)")
 
 
-def kernel_name(kbd, tune=193):
+def kernel_names(kbd):
+    """Mangled names of the batch kernel: march_persistent_kernel<KBD, false, kOutLinear>, and the same kernel in
+    checkouts that still carry the top-grid and tuning parameters (<KBD, false, false, kOutLinear, 193>)."""
     kb = f"Li{kbd}E" if kbd >= 0 else f"Lin{-kbd}E"
-    return f"_ZN3vrb23march_persistent_kernelI{kb}Lb0ELb0ELi0ELi{tune}EEEvNS_9LaunchDevE"
+    return [f"_ZN3vrb23march_persistent_kernelI{kb}Lb0ELi0EEEvNS_9LaunchDevE",
+            f"_ZN3vrb23march_persistent_kernelI{kb}Lb0ELb0ELi0ELi193EEEvNS_9LaunchDevE"]
 
 
 def compile_cubin(src, kbd, out_dir, extra):
@@ -49,7 +52,7 @@ def compile_cubin(src, kbd, out_dir, extra):
     cubin = os.path.join(out_dir, f"vr_kernels_{kbd}.cubin")
     cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
            "-I" + os.path.join(src, "include"), "-I" + os.path.join(src, "volrend_b200", "csrc"),
-           "-diag-suppress", "20012", "-DVR_BLOCK=128", "-DVR_MINB=8", "-DVR_TW=4", f"-DVR_KBD={kbd}",
+           "-diag-suppress", "20012", f"-DVR_KBD={kbd}",
            "-Xptxas", "-v", "-cubin", os.path.join(src, "volrend_b200", "csrc", "vr_kernels_inst.cu"), "-o", cubin]
     cmd += extra
     r = subprocess.run(cmd, capture_output=True, text=True)
@@ -91,9 +94,9 @@ def branch_target(text):
 def blocks(ins):
     addr = [a for a, _ in ins]
     pos = {a: i for i, a in enumerate(addr)}
-    recs = [i for i, (_, t) in enumerate(ins) if "LDG.E.NA.128" in t]
+    recs = [i for i, (_, t) in enumerate(ins) if "LDG.E.128.CONSTANT" in t]
     if not recs:
-        sys.exit("no colour-record loads (LDG.E.NA.128) in the kernel")
+        sys.exit("no colour-record loads (LDG.E.128.CONSTANT) in the kernel")
     loops = []   # (head index, back-edge index)
     fwd = []     # (branch index, target index)
     for i, (a, t) in enumerate(ins):
@@ -151,8 +154,10 @@ def main():
     os.makedirs(out_dir, exist_ok=True)
     try:
         for kbd in [int(k) for k in a.kbd.split(",")]:
-            name = kernel_name(kbd)
             cubin, log = compile_cubin(os.path.abspath(a.src), kbd, out_dir, a.extra)
+            name = next((n for n in kernel_names(kbd) if f"Function properties for {n}" in log), None)
+            if name is None:
+                sys.exit(f"no batch kernel for KBD={kbd} in {cubin}")
             regs, frame, sst, sld = ptxas_stats(log, name)
             ins = disassemble(cubin, name)
             if a.keep:
@@ -160,7 +165,7 @@ def main():
                     f.writelines(f"{ad:05x}  {t}\n" for ad, t in ins)
             b = blocks(ins)
             r = b["ranges"]
-            print(f"KBD={kbd}  march_persistent_kernel<{kbd}, false, false, kOutLinear, 193>")
+            print(f"KBD={kbd}  march_persistent_kernel<{kbd}, false, kOutLinear>")
             print(f"  registers {regs}, stack frame {frame} B, spill stores {sst} B, spill loads {sld} B")
             print(f"  march loop  {b['loop']:4d}  [{r['loop'][0]:#x}, {r['loop'][1]:#x}]")
             print(f"  body        {b['body']:4d}  (empty sample, one table fetch)")

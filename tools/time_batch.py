@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One timing line for the current library build / environment (VR_LIB_SUFFIX, VR_EXTRA_SMEM, ...):
+"""One timing line for one kernel variant:
 200-view batch and back-to-back single-frame launches on the bench tree (cached as an .npz in /tmp).
 usage: time_batch.py [label] [variant] [depth] [basis]"""
 import ctypes as C

@@ -10,8 +10,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# VR_LIB_SUFFIX selects a tuning build (e.g. "_b128m7", see Makefile); default is the product build
-LIB_PATH = os.path.join(_HERE, "libvolrend_b200" + os.environ.get("VR_LIB_SUFFIX", "") + ".so")
+LIB_PATH = os.path.join(_HERE, "libvolrend_b200.so")
 
 VR_BASIS_MAX = 25
 VR_OK, VR_EINVAL, VR_ENODEVICE, VR_ECUDA, VR_ENOMEM, VR_EUNSUPPORTED = 0, -1, -2, -3, -4, -5

@@ -41,8 +41,6 @@ thread_local std::string g_err;
 std::atomic<int> g_variant{0};
 std::atomic<unsigned long long> g_launches{0};
 std::atomic<int> g_max_ctas{0};
-// Resolved default variants (vr_kernels.h): queue kernel for >= 4 basis functions, else inline shading
-constexpr int kVariantQueue = 7, kVariantInline = 3 + 16 * 193;
 constexpr int kQueueSlots = 256;
 constexpr int kCamRing = 8192;  // device ring of per-view cameras for batched launches
 }  // namespace
@@ -125,8 +123,6 @@ struct StreamRes {
     OptDev* opt_ring = nullptr;      // kCamRing entries beside cam_ring (same slots), allocated by the first
                                      // batch with options per view
     unsigned int next_queue = 0, cam_pos = 0;
-    unsigned char* pool = nullptr;   // parked-ray stacks of the ray-pool kernel (kind 8), allocated on first use
-    size_t pool_bytes = 0;
 };
 
 struct vr_tree {
@@ -136,10 +132,8 @@ struct vr_tree {
     uint32_t* wide = nullptr;
     unsigned char* wrecs = nullptr;
     float* extra = nullptr;
-    // slot-indexed arrays: only the experiment kernels (-DVR_EXPERIMENTS) read them
+    // upload scratch (slot-indexed node words, table entry -> slot), freed once the tables are built
     uint32_t* nodes = nullptr;
-    unsigned char* recs = nullptr;
-    uint32_t* top = nullptr;
     uint32_t* wslot = nullptr;
     long long n_tables = 0;
     std::mutex res_mu;
@@ -156,7 +150,6 @@ struct vr_tree {
     std::mutex host_mu;
     vr_tree_info info{};
     int data_dim = 0;
-    size_t l2_window_bytes = 0;  // table window kept in persisting L2 (VR_L2_PERSIST=1)
     // grid wireframe (vr_tree_wireframe): cells per level, counted on the first call
     std::mutex wire_mu;
     bool wire_ready = false;
@@ -412,49 +405,6 @@ __global__ void build_wrecs_kernel(const uint32_t* __restrict__ wslot, LeafSrc S
     reinterpret_cast<uint4*>(wrecs + (size_t)e * rec_bytes)[c] = v;
 }
 
-#ifdef VR_EXPERIMENTS
-// recs[i]: colour coefficients of slot i, padded.  One thread per (slot, 16-byte chunk).
-__global__ void relayout_recs_kernel(LeafSrc S, unsigned char* __restrict__ recs, int rec_bytes) {
-    const int chunks = rec_bytes >= 16 ? rec_bytes / 16 : 1;
-    const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long slot = gid / chunks;
-    const int c = (int)(gid % chunks);
-    if (slot >= S.n_slots) return;
-    if (rec_bytes == 8) {
-        ushort4 v;
-        v.x = leaf_half(S, slot, 0); v.y = leaf_half(S, slot, 1); v.z = leaf_half(S, slot, 2); v.w = 0;
-        reinterpret_cast<ushort4*>(recs)[slot] = v;
-        return;
-    }
-    unsigned short h[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) h[j] = leaf_half(S, slot, c * 8 + j);
-    uint4 v;
-    v.x = h[0] | ((uint32_t)h[1] << 16); v.y = h[2] | ((uint32_t)h[3] << 16);
-    v.z = h[4] | ((uint32_t)h[5] << 16); v.w = h[6] | ((uint32_t)h[7] << 16);
-    reinterpret_cast<uint4*>(recs + (size_t)slot * rec_bytes)[c] = v;
-}
-
-// top[cell]: leaf word (bit31 | depth<<28 | sigma) or the depth-4 node id.
-__global__ void build_top_kernel(const uint32_t* __restrict__ nodes, uint32_t* __restrict__ top) {
-    const int cell = blockIdx.x * blockDim.x + threadIdx.x;
-    if (cell >= kTopCells) return;
-    const uint32_t cx = (cell >> 8) & 15, cy = (cell >> 4) & 15, cz = cell & 15;
-    uint32_t node = 0;
-    for (int l = 1; l <= kTopLevel; ++l) {
-        const int sh = kTopLevel - l;
-        const uint32_t oct = (((cx >> sh) & 1u) << 2) | (((cy >> sh) & 1u) << 1) | ((cz >> sh) & 1u);
-        const uint32_t w = nodes[node * 8u + oct];
-        if (w & kLeafBit) {
-            top[cell] = kLeafBit | ((uint32_t)l << 28) | (w & 0xffffu);
-            return;
-        }
-        node = w;
-    }
-    top[cell] = node;
-}
-#endif
-
 // one block per queue slot: {head, done} = 0, every SM's block state = "no block", locks free (vr_march.cuh next_item)
 __global__ void queue_init_kernel(unsigned char* slots) {
     unsigned char* slot = slots + (size_t)blockIdx.x * kQueueSlotBytes;
@@ -493,7 +443,6 @@ int vr_tree_variant(const vr_tree* t) {
     if (!t) return -1;
     const int v = g_variant.load();
     if (v != 0) return variant_ok(t->dev.kbd, v) ? v : -1;
-    (void)kVariantQueue;   // single-view launches of 4/9/16-basis trees use it (launch_march, vr_kernels_inst.cu)
     return kVariantInline;
 }
 unsigned long long vr_launch_count(void) { return g_launches.load(); }
@@ -512,9 +461,9 @@ void vr_tree_destroy(vr_tree* t) {
     int prev = 0;
     cudaGetDevice(&prev);
     cudaSetDevice(t->device);
-    cudaFree(t->nodes); cudaFree(t->recs); cudaFree(t->top); cudaFree(t->extra);
+    cudaFree(t->nodes); cudaFree(t->extra);
     cudaFree(t->wide); cudaFree(t->wslot); cudaFree(t->wrecs);
-    for (auto& kv : t->res) { cudaFree(kv.second.queues); cudaFree(kv.second.cam_ring); cudaFree(kv.second.opt_ring); cudaFree(kv.second.pool); }
+    for (auto& kv : t->res) { cudaFree(kv.second.queues); cudaFree(kv.second.cam_ring); cudaFree(kv.second.opt_ring); }
     for (int i = 0; i < vr_tree::HostPath::kRing; ++i) {
         cudaFree(t->host.buf[i]);
         if (t->host.rendered[i]) cudaEventDestroy(t->host.rendered[i]);
@@ -686,28 +635,15 @@ static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, 
         build_wrecs_kernel<<<(unsigned)((rwork + TB - 1) / TB), TB>>>(t->wslot, S, t->wrecs, n_entries, rec_bytes);
         VR_CUDA(cudaGetLastError());
     }
-#ifdef VR_EXPERIMENTS
-    {   // slot-indexed records and the dense top grid of the experiment kernels
-        VR_CUDA(cudaMalloc(&t->recs, (size_t)n_slots * rec_bytes));
-        VR_CUDA(cudaMalloc(&t->top, kTopCells * 4));
-        const long long rec_work = n_slots * (rec_bytes >= 16 ? rec_bytes / 16 : 1);
-        relayout_recs_kernel<<<(unsigned)((rec_work + TB - 1) / TB), TB>>>(S, t->recs, rec_bytes);
-        build_top_kernel<<<(kTopCells + TB - 1) / TB, TB>>>(t->nodes, t->top);
-        VR_CUDA(cudaGetLastError());
-    }
     VR_CUDA(cudaDeviceSynchronize());
-#else
-    VR_CUDA(cudaDeviceSynchronize());
-    // the product kernels read the tables and the table-indexed records only
+    // the kernels read the tables and the table-indexed records only
     cudaFree(t->nodes); t->nodes = nullptr;
     cudaFree(t->wslot); t->wslot = nullptr;
-#endif
     t->n_tables = n_tab;
     g_launches += 7;
 
     TreeDev& D = t->dev;
-    D.nodes = t->nodes; D.recs = t->recs; D.top = t->top; D.extra = t->extra;
-    D.wide = t->wide; D.wslot = t->wslot; D.wrecs = t->wrecs;
+    D.wide = t->wide; D.wrecs = t->wrecs; D.extra = t->extra;
     for (int i = 0; i < 3; ++i) { D.offset[i] = d->offset[i]; D.scale[i] = d->scale[i]; }
     D.ndc_width = d->use_ndc ? d->ndc_width : -1.f;  // data_spec.hpp:47
     D.ndc_height = d->ndc_height; D.ndc_focal = d->ndc_focal;
@@ -719,25 +655,11 @@ static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, 
     vr_tree_info& I = t->info;
     I.capacity = d->capacity; I.max_depth = D.max_depth; I.rec_bytes = rec_bytes;
     I.node_bytes = n_slots * 4; I.rec_total_bytes = n_slots * (long long)rec_bytes;
-    I.top_bytes = kTopCells * 4;
+    I.top_bytes = 16 * 16 * 16 * 4;   // a dense 16^3 grid of node words
     I.kernel_basis = kbd; I.wide_parity = wp; I.n_tables = n_tab;
     I.wide_bytes = n_entries * 4; I.wrecs_bytes = n_entries * (long long)rec_bytes;
     I.kernel_bytes = I.wide_bytes + I.wrecs_bytes;
-    I.device_bytes = I.kernel_bytes + (t->nodes ? I.node_bytes : 0) + (t->recs ? I.rec_total_bytes : 0) +
-                     (t->wslot ? I.wide_bytes : 0) + (t->top ? I.top_bytes : 0);
-    if (const char* e = getenv("VR_L2_PERSIST")) {
-        if (atoi(e) > 0) {
-            int max_persist = 0, max_window = 0;
-            cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, t->device);
-            cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, t->device);
-            size_t want = (size_t)n_entries * 4;
-            if (want > (size_t)max_window) want = (size_t)max_window;
-            size_t carve = want < (size_t)max_persist ? want : (size_t)max_persist;
-            if (carve > 0 && cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve) == cudaSuccess)
-                t->l2_window_bytes = want;
-            cudaGetLastError();
-        }
-    }
+    I.device_bytes = I.kernel_bytes;
     guard.ok = true;
     *out = t;
     return VR_OK;
@@ -812,24 +734,6 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
         std::lock_guard<std::mutex> lk(mt->res_mu);
         cfg.queue = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(sr->queues) + (size_t)(sr->next_queue++ % kQueueSlots) * kQueueSlotBytes);
     }
-    cfg.pool = nullptr; cfg.pool_bytes = 0;
-    if ((cfg.variant & 15) == 8) {   // ray-pool kernel: its parked-ray stacks live with the (tree, stream) resources
-        const size_t need = with_kbd(t->dev.kbd, size_t(0), [&](auto k) {
-            return pool_bytes_for<decltype(k)::value>(t->num_sms, t->dev.max_depth);
-        });
-        std::lock_guard<std::mutex> lk(mt->res_mu);
-        if (need > sr->pool_bytes) {
-            // a grow only happens before the first kind-8 launch on this stream (the size depends on the tree alone)
-            if (sr->pool) { cudaStreamSynchronize(stream); cudaFree(sr->pool); sr->pool = nullptr; sr->pool_bytes = 0; }
-            if (cudaMalloc(&sr->pool, need) == cudaSuccess) sr->pool_bytes = need;
-            else { cudaGetLastError(); sr->pool = nullptr; }   // no memory: the kernel runs without parking
-        }
-        cfg.pool = sr->pool; cfg.pool_bytes = sr->pool_bytes;
-    }
-    cfg.l2_window = t->wide;
-    cfg.l2_window_bytes = t->l2_window_bytes;
-    static const bool no_pdl = getenv("VR_NO_PDL") != nullptr && atoi(getenv("VR_NO_PDL")) > 0;
-    cfg.pdl = !no_pdl;
     // variant_ok above has rejected every kbd without kernels
     const cudaError_t e = with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
         return launch_march<decltype(k)::value>(P, cfg);

@@ -6,12 +6,11 @@
 
 namespace vrb {
 
-// variant = kind + 16 * tune; 0 = the default for the tree's basis size.
-//   kind 7: persistent warps + warp-shared shading queue (vr_march_q.cuh), >= 4 basis functions
-//   kind 8: kind 7 + ray pool (tails of tiles are parked and re-marched 32 at a time), >= 4 basis functions
-//   kind 3, tune 193: persistent warps, inline shading (vr_march.cuh)
-//   -DVR_EXPERIMENTS only: 1 tile kernel, 2 tile + TMA top grid, 3 persistent (+ tuning bits),
-//   4 persistent + TMA top grid, 5 persistent + deferred shading, 6 same + TMA top grid
+// Kernel variants (vr_set_variant); 0 = the default for the launch and the tree's basis size.
+//   kVariantQueue:  persistent warps + warp-shared shading queue (vr_march_q.cuh), >= 4 basis functions
+//   kVariantInline: persistent warps, inline shading (vr_march.cuh); its id, 3 + 16 * 193, stays what callers set
+constexpr int kVariantQueue = 7, kVariantInline = 3 + 16 * 193;
+
 struct LaunchCfg {
     int variant;
     int max_ctas;    // > 0: cap the persistent grid (leaves SMs to a concurrent copy/collective kernel)
@@ -19,11 +18,6 @@ struct LaunchCfg {
     bool surface;    // write a cudaSurfaceObject instead of linear memory
     int num_sms;
     unsigned int* queue;  // persistent kernels: {work head, done CTAs}
-    unsigned char* pool;  // kind 8: parked-ray stacks of this (tree, stream), pool_bytes large (see pool_bytes_for)
-    size_t pool_bytes;
-    const void* l2_window;   // optional persisting-L2 access window (the node table)
-    size_t l2_window_bytes;  // 0 = none
-    bool pdl;                // allow overlap with the previous launch of the stream (see vr_march.cuh)
     cudaStream_t stream;
 };
 
@@ -33,10 +27,6 @@ cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg);
 template <int KBD>
 bool variant_supported(int variant);
 
-// bytes of parked-ray storage a kind-8 launch needs on a device with num_sms SMs (0 when KBD has no such kernel)
-template <int KBD>
-size_t pool_bytes_for(int num_sms, int max_depth);
-
 extern template cudaError_t launch_march<-1>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<1>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<4>(LaunchDev&, const LaunchCfg&);
@@ -44,16 +34,10 @@ extern template cudaError_t launch_march<9>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<16>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<25>(LaunchDev&, const LaunchCfg&);
 extern template bool variant_supported<-1>(int);
-extern template size_t pool_bytes_for<-1>(int, int);
 extern template bool variant_supported<1>(int);
-extern template size_t pool_bytes_for<1>(int, int);
 extern template bool variant_supported<4>(int);
-extern template size_t pool_bytes_for<4>(int, int);
 extern template bool variant_supported<9>(int);
-extern template size_t pool_bytes_for<9>(int, int);
 extern template bool variant_supported<16>(int);
-extern template size_t pool_bytes_for<16>(int, int);
 extern template bool variant_supported<25>(int);
-extern template size_t pool_bytes_for<25>(int, int);
 
 }  // namespace vrb

@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(kQBlock) query_kernel(const QueryLaunch Q) {
                 const uint32_t e = descend_wide(Q.tree, u, j, T, wl, &s_tab[0][threadIdx.x], kQBlock);
                 pu[0] = u[0]; pu[1] = u[1]; pu[2] = u[2];
                 pstep = j;
-                if (need_rec) load_rec<KBD, kTuneHint | kTuneRec32>(rec_addr(Q.tree.wrecs, e, RecBytes<KBD>::n), rw);
+                if (need_rec) load_rec<KBD>(rec_addr(Q.tree.wrecs, e, RecBytes<KBD>::n), rw);
                 if constexpr (EVAL) {
                     if (Q.sigma) Q.sigma[i] = __half2float(__ushort_as_half((unsigned short)(wl & 0xffffu)));
                     if (Q.rgb) {

@@ -9,40 +9,23 @@ namespace vrb {
 
 // Leaf flag of a node word; the low 16 bits then hold sigma as fp16 bits.
 constexpr uint32_t kLeafBit = 0x80000000u;
-// Level of the dense top grid staged into shared memory (16^3 cells).
-constexpr int kTopLevel = 4;
-constexpr int kTopCells = 1 << (3 * kTopLevel);
 // Deepest leaf we accept: positions are 24-bit fixed point (fp32 mantissa).
 constexpr int kMaxTreeDepth = 23;
-// Octree levels resolved per table fetch (2: 64-entry tables, 3: 512-entry tables).  Build-time choice so that entry
-// indices are shifts by constants: make lib EXTRA=-DVR_WIDE_LV=3.
-#ifndef VR_WIDE_LV
-#define VR_WIDE_LV 2
-#endif
-constexpr int kWideLv = VR_WIDE_LV;
+// Octree levels resolved per table fetch: 64-entry tables.
+constexpr int kWideLv = 2;
 constexpr int kWideEntries = 1 << (3 * kWideLv);
-static_assert(kWideLv == 2 || kWideLv == 3, "tables resolve two or three octree levels");
 // tables on a root-to-leaf path (the ancestor stack of the march kernels)
 inline __host__ __device__ int wide_table_levels(int max_depth) { return (max_depth + kWideLv - 2) / kWideLv + 1; }
 
-// Device copy of one N3Tree, re-laid-out at upload (vr_tree_create):
-//  nodes[node*8 + oct]  internal: absolute child node id (>0)
-//                       leaf:     kLeafBit | sigma_fp16_bits
-//  recs[(node*8+oct)*rec_bytes ...]  colour coefficients only (sigma moved into the
-//                       node word), channel-major fp16, padded to a 16-byte multiple
-//                       (8 bytes for one coefficient per channel)
-//  top[cell]            16^3 dense grid: (depth<<28)|node of the deepest internal node
-//                       (depth <= kTopLevel-1) on the path to that level-4 cell
+// Device copy of one N3Tree, re-laid-out at upload (vr_tree_create).
 struct TreeDev {
-    const uint32_t* nodes;
-    const unsigned char* recs;
-    const uint32_t* top;
-    // two-levels-per-step view of the same octree: one 64-entry table per internal node whose depth has
+    // two-levels-per-step view of the octree: one 64-entry table per internal node whose depth has
     // parity wide_p (plus the root); entry = table id of the grandchild, or leaf word:
     //   kLeafBit | (103 + leaf depth) << 23 | sigma   (bits 23..30 = fp32 exponent of the cube size)
     const uint32_t* wide;
-    const uint32_t* wslot;   // parallel array: the leaf's slot (node*8+oct) for record lookup
-    const unsigned char* wrecs;  // colour records re-indexed by wide entry (no wslot indirection)
+    // colour records indexed by table entry: coefficients only (sigma is in the leaf word), channel-major fp16,
+    // padded to a 16-byte multiple (8 bytes for one coefficient per channel)
+    const unsigned char* wrecs;
     const float* extra;
     float offset[3];
     float scale[3];
@@ -121,7 +104,6 @@ struct LaunchDev {
     // share a block, so that neighbouring tiles of neighbouring poses -- same tables, same records -- are marched at the
     // same time on the same L1.  blk_mode 0: one tile per queue item (single frames: finest balance).
     int32_t blk_mode, blocks_x, n_blocks, blk_gshift, blk_wshift, blk_groups;   // blk_groups: view groups of the batch
-    unsigned char* pool;                // ray-pool kernels: parked-ray stacks, one per CTA (vr_march_q.cuh); nullptr = no parking
     unsigned long long* trace;          // diagnostics: per work item {start ns, end ns, smid, warp}
     // per-view options (vr_render_batch_opts): device array of n_views entries, read only by the kOutViewOpts
     // instantiations; nullptr = every view uses `opt`.  Last field, so the other fields keep their offsets.
