@@ -69,10 +69,12 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp volrend_b200/csrc/vr_frames.h incl
 $(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
-oracle: oracle/liboracle.so oracle/libprobe_oracle.so
+oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so
 oracle/liboracle.so: oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 oracle/libprobe_oracle.so: oracle/probe_oracle.c oracle/march_oracle.c oracle/march_oracle.h
+	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
+oracle/libweights_oracle.so: oracle/weights_oracle.c oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 
 ref:
@@ -88,4 +90,4 @@ shim:
 	 else echo "reference tree $(VOLREND_REF) not present: shim needs the reference headers"; fi
 
 clean:
-	rm -rf build $(LIB) oracle/liboracle.so oracle/_ref
+	rm -rf build $(LIB) oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/_ref

@@ -129,6 +129,14 @@ void vr_default_options(vr_options* o);
 
 int vr_tree_create(const vr_tree_desc* desc, vr_tree** out);
 int vr_tree_create_quantized(const vr_tree_quant_desc* desc, vr_tree** out);
+/* The same with creation flags; flags = 0 is vr_tree_create / vr_tree_create_quantized, other bits are VR_EINVAL.
+ * VR_TREE_SLOT_MAP keeps the table entry -> slot map the upload builds (one u32 per table entry: node * 8 + octant of
+ * the entry's leaf in the source child / data arrays, or 0xffffffff for an entry that is not a leaf), which
+ * vr_tree_leaf_weights needs.  With it, device_bytes includes the map (4 bytes per table entry); kernel_bytes and the
+ * march kernels are the same. */
+#define VR_TREE_SLOT_MAP 1u
+int vr_tree_create_ex(const vr_tree_desc* desc, uint32_t flags, vr_tree** out);
+int vr_tree_create_quantized_ex(const vr_tree_quant_desc* desc, uint32_t flags, vr_tree** out);
 void vr_tree_destroy(vr_tree* tree);
 int vr_tree_get_info(const vr_tree* tree, vr_tree_info* info);
 
@@ -151,6 +159,22 @@ int vr_render_batch(const vr_tree* tree, const vr_camera* cams, int n_views, con
  * Used by the animator (volrend_anim, main_anim.cpp:268-307), whose interpolated options change every frame. */
 int vr_render_batch_opts(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opts,
                          const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev,
+                         void* stream);
+
+/* Maximum compositing weight per leaf over n_views views (the weight-based pruning of the PlenOctree conversion).
+ * Every shaded sample (sigma > sigma_thresh) of every pixel of `tile` (NULL = full frame) of every view sets
+ *   weight_dev[slot] = max(weight_dev[slot], T * (1 - att))
+ * with the weight computed by exactly the operations of vr_render_batch's march; slot = node * 8 + octant of the
+ * sample's leaf in the source arrays.  weight_dev: capacity * 8 floats on the tree's device, initialised by the caller
+ * (e.g. to -inf), so that calls accumulate and one call over a set of views equals several calls over any split of it.
+ * The maximum is taken in the total order of floats with -0 < +0 (negative weights arise when sigma_thresh < 0 lets
+ * sigma <= 0 through); NaN weights are not recorded.  Of `opt`, step_size, sigma_thresh, stop_thresh and render_bbox
+ * act as in vr_render_batch (so do NDC and early termination); render_depth, basis_minmax, rot_dirs and
+ * background_brightness have no effect.  alpha_dev (NULL, or tile-sized floats per view) receives each ray's alpha,
+ * the alpha channel of vr_render_batch's float output; counters_dev accumulates the usual counters.  Asynchronous on
+ * stream.  VR_EUNSUPPORTED for a tree created without VR_TREE_SLOT_MAP; otherwise validated as vr_render_batch. */
+int vr_tree_leaf_weights(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
+                         const vr_rect* tile, float* weight_dev, float* alpha_dev, vr_counters* counters_dev,
                          void* stream);
 
 /* launch_renderer(offscreen=false): rgba8_dev is read (existing colour) and overwritten;

@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libvolrend_b200.so")
 VR_BASIS_MAX = 25
 VR_OK, VR_EINVAL, VR_ENODEVICE, VR_ECUDA, VR_ENOMEM, VR_EUNSUPPORTED = 0, -1, -2, -3, -4, -5
 VR_FMT_RGBA, VR_FMT_SH, VR_FMT_SG, VR_FMT_ASG = 0, 1, 2, 3
+VR_TREE_SLOT_MAP = 1
 
 
 class vr_tree_desc(C.Structure):
@@ -68,6 +69,10 @@ SYMBOLS = {
     "vr_default_options": (None, [C.POINTER(vr_options)]),
     "vr_tree_create": (C.c_int, [C.POINTER(vr_tree_desc), C.POINTER(C.c_void_p)]),
     "vr_tree_create_quantized": (C.c_int, [C.POINTER(vr_tree_quant_desc), C.POINTER(C.c_void_p)]),
+    "vr_tree_create_ex": (C.c_int, [C.POINTER(vr_tree_desc), C.c_uint32, C.POINTER(C.c_void_p)]),
+    "vr_tree_create_quantized_ex": (C.c_int, [C.POINTER(vr_tree_quant_desc), C.c_uint32, C.POINTER(C.c_void_p)]),
+    "vr_tree_leaf_weights": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
+                                       C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_tree_destroy": (None, [C.c_void_p]),
     "vr_tree_get_info": (C.c_int, [C.c_void_p, C.POINTER(vr_tree_info)]),
     "vr_render": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.POINTER(vr_options), C.POINTER(vr_rect),

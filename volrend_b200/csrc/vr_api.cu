@@ -132,7 +132,8 @@ struct vr_tree {
     uint32_t* wide = nullptr;
     unsigned char* wrecs = nullptr;
     float* extra = nullptr;
-    // upload scratch (slot-indexed node words, table entry -> slot), freed once the tables are built
+    // upload scratch (slot-indexed node words, table entry -> slot), freed once the tables are built; with
+    // VR_TREE_SLOT_MAP the table entry -> slot map stays (vr_tree_leaf_weights)
     uint32_t* nodes = nullptr;
     uint32_t* wslot = nullptr;
     long long n_tables = 0;
@@ -475,9 +476,10 @@ void vr_tree_destroy(vr_tree* t) {
     delete t;
 }
 
-static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, vr_tree** out) {
+static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, uint32_t create_flags, vr_tree** out) {
     if (!d || !out) return fail(VR_EINVAL, "null argument");
     *out = nullptr;
+    if (create_flags & ~(uint32_t)VR_TREE_SLOT_MAP) return fail(VR_EINVAL, "unknown tree flags 0x%x", create_flags);
     if (int rc = need_device(nullptr)) return rc;
     if (d->N != 2) return fail(VR_EUNSUPPORTED, "N=%d: only N=2 octrees are supported (as in the reference)", d->N);
     if (d->capacity < 1 || d->capacity >= (1ll << 28)) return fail(VR_EINVAL, "capacity %lld out of range", (long long)d->capacity);
@@ -636,9 +638,10 @@ static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, 
         VR_CUDA(cudaGetLastError());
     }
     VR_CUDA(cudaDeviceSynchronize());
-    // the kernels read the tables and the table-indexed records only
+    // the march kernels read the tables and the table-indexed records only; the weights pass also the slot map
     cudaFree(t->nodes); t->nodes = nullptr;
-    cudaFree(t->wslot); t->wslot = nullptr;
+    const bool slot_map = (create_flags & VR_TREE_SLOT_MAP) != 0;
+    if (!slot_map) { cudaFree(t->wslot); t->wslot = nullptr; }
     t->n_tables = n_tab;
     g_launches += 7;
 
@@ -659,19 +662,23 @@ static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, 
     I.kernel_basis = kbd; I.wide_parity = wp; I.n_tables = n_tab;
     I.wide_bytes = n_entries * 4; I.wrecs_bytes = n_entries * (long long)rec_bytes;
     I.kernel_bytes = I.wide_bytes + I.wrecs_bytes;
-    I.device_bytes = I.kernel_bytes;
+    I.device_bytes = I.kernel_bytes + (slot_map ? n_entries * 4 : 0);
     guard.ok = true;
     *out = t;
     return VR_OK;
 }
 
-int vr_tree_create(const vr_tree_desc* d, vr_tree** out) { return tree_create_impl(d, nullptr, out); }
+int vr_tree_create_ex(const vr_tree_desc* d, uint32_t flags, vr_tree** out) {
+    return tree_create_impl(d, nullptr, flags, out);
+}
+int vr_tree_create(const vr_tree_desc* d, vr_tree** out) { return vr_tree_create_ex(d, 0, out); }
 
-int vr_tree_create_quantized(const vr_tree_quant_desc* q, vr_tree** out) {
+int vr_tree_create_quantized_ex(const vr_tree_quant_desc* q, uint32_t flags, vr_tree** out) {
     if (!q) return fail(VR_EINVAL, "null argument");
     if (q->base.data) return fail(VR_EINVAL, "quantised descriptor must not carry decoded data");
-    return tree_create_impl(&q->base, q, out);
+    return tree_create_impl(&q->base, q, flags, out);
 }
+int vr_tree_create_quantized(const vr_tree_quant_desc* q, vr_tree** out) { return vr_tree_create_quantized_ex(q, 0, out); }
 
 int vr_tree_get_info(const vr_tree* t, vr_tree_info* info) {
     if (!t || !info) return fail(VR_EINVAL, "null argument");
@@ -720,10 +727,11 @@ int stream_res(vr_tree* t, cudaStream_t stream, StreamRes*& out) {
     return VR_OK;
 }
 
-int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStream_t stream) {
+// weights: the weights pass (one kernel for every basis size, whatever the variant setting)
+int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStream_t stream, bool weights = false) {
     LaunchCfg cfg;
     cfg.variant = vr_get_variant();
-    if (!variant_ok(t->dev.kbd, cfg.variant))
+    if (!weights && !variant_ok(t->dev.kbd, cfg.variant))
         return fail(VR_EUNSUPPORTED, "kernel variant %d is not available for kernel basis %d", cfg.variant, t->dev.kbd);
     cfg.max_ctas = g_max_ctas.load();
     cfg.count = count; cfg.surface = surface; cfg.num_sms = t->num_sms; cfg.stream = stream;
@@ -735,7 +743,7 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
         cfg.queue = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(sr->queues) + (size_t)(sr->next_queue++ % kQueueSlots) * kQueueSlotBytes);
     }
     // variant_ok above has rejected every kbd without kernels
-    const cudaError_t e = with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
+    const cudaError_t e = weights ? launch_weights(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
         return launch_march<decltype(k)::value>(P, cfg);
     });
     if (e != cudaSuccess) return fail(VR_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
@@ -801,8 +809,9 @@ int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_
 // hold h rows of w pixels per view); this adds the tree, the cameras and the options, and launches the views in chunks
 // that fit the camera ring and the 31-bit tile index, the output pointers advanced to each chunk's first view.
 // opt_stride as in vr_frames.h; a chunk of one view is an ordinary single-view launch with that view's options.
+// weights: the weights pass, P.alpha advanced like the outputs.
 int march(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
-          const LaunchDev& P, bool surface, cudaStream_t stream) {
+          const LaunchDev& P, bool surface, cudaStream_t stream, bool weights = false) {
     const long long tb = tile_bound(vr_rect{P.x0, P.y0, P.w, P.h});
     const int max_views = tb * kCamRing > 0x7fffffffLL ? (int)(0x7fffffffLL / tb) : kCamRing;
     const size_t px = (size_t)P.w * P.h;
@@ -816,8 +825,9 @@ int march(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options
         C.rgba8 = skip(P.rgba8, 4 * px * v0);
         C.rgbaf = skip(P.rgbaf, px * v0);
         C.depth_in = skip(P.depth_in, px * v0);
+        C.alpha = skip(P.alpha, px * v0);
         if (int rc = stage_cams(t, cams + v0, nv, stream, C, opt_stride ? o : nullptr)) return rc;
-        return dispatch(t, C, P.counters != nullptr, surface, stream);
+        return dispatch(t, C, P.counters != nullptr, surface, stream, weights);
     });
 }
 
@@ -874,6 +884,26 @@ int vr_render_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, c
                          const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev,
                          void* stream) {
     return render_batch(t, cams, n_views, opts, 1, tile, rgba8_dev, rgba32f_dev, counters_dev, stream);
+}
+
+int vr_tree_leaf_weights(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
+                         const vr_rect* tile, float* weight_dev, float* alpha_dev, vr_counters* counters_dev,
+                         void* stream) {
+    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
+    if (n_views == 0) return VR_OK;
+    if (!weight_dev) return fail(VR_EINVAL, "null weight buffer");
+    vr_rect r;
+    int rc = check_common(t, cams, opt, tile, r);
+    if (rc) return rc;
+    if ((rc = same_size(cams, n_views))) return rc;
+    if (!t->wslot)
+        return fail(VR_EUNSUPPORTED, "leaf weights need the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if (r.w == 0 || r.h == 0) return VR_OK;
+    LaunchDev P{};
+    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
+    P.counters = counters_dev;
+    P.wslot = t->wslot; P.weights = weight_dev; P.alpha = alpha_dev;
+    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, true);
 }
 
 int vr_render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,

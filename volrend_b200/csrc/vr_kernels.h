@@ -27,6 +27,10 @@ cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg);
 template <int KBD>
 bool variant_supported(int variant);
 
+// The weights pass of vr_tree_leaf_weights: the inline-shading kernel's kOutWeights instantiation (vr_march.cuh).  It
+// reads no colour record, so one kernel serves every basis size; it is built in the VR_KBD=1 object.
+cudaError_t launch_weights(LaunchDev& P, const LaunchCfg& cfg);
+
 extern template cudaError_t launch_march<-1>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<1>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<4>(LaunchDev&, const LaunchCfg&);

@@ -8,7 +8,8 @@
 //                      RGBA / 1 / 25 basis functions, and the A/B partner of the queue kernel in the parity tests
 //                      and the bench
 // Both also come as kOutViewOpts instantiations (plain and counting), which read each view's options from
-// LaunchDev::opts: batches with options per view.
+// LaunchDev::opts: batches with options per view.  The VR_KBD=1 object also holds the weights pass
+// (march_persistent_kernel<0, *, kOutWeights>, vr_tree_leaf_weights), one kernel for every basis size.
 #include <mutex>
 
 #include "vr_kernels.h"
@@ -144,5 +145,14 @@ cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg) {
 
 template cudaError_t launch_march<VR_KBD>(LaunchDev&, const LaunchCfg&);
 template bool variant_supported<VR_KBD>(int);
+
+#if VR_KBD == 1
+// KBD 0: no basis set-up and no parked ray constants (the weights march reads no record)
+cudaError_t launch_weights(LaunchDev& P, const LaunchCfg& cfg) {
+    const size_t smem = march_smem_bytes(P.tree.max_depth);
+    if (cfg.count) return launch_persistent_grid(march_persistent_kernel<0, true, kOutWeights>, smem, P, cfg);
+    return launch_persistent_grid(march_persistent_kernel<0, false, kOutWeights>, smem, P, cfg);
+}
+#endif
 
 }  // namespace vrb

@@ -108,6 +108,12 @@ struct LaunchDev {
     // per-view options (vr_render_batch_opts): device array of n_views entries, read only by the kOutViewOpts
     // instantiations; nullptr = every view uses `opt`.  Last field, so the other fields keep their offsets.
     const OptDev* opts;
+    // leaf weights (vr_tree_leaf_weights), read only by the kOutWeights instantiations: the tree's table entry -> slot
+    // map, the caller's per-slot maximum weights and the per-pixel alpha output (or nullptr).  After `opts`, so that
+    // every other field keeps its offset.
+    const uint32_t* wslot;
+    float* weights;
+    float* alpha;
 };
 
 }  // namespace vrb

@@ -91,6 +91,7 @@ class N3Tree:
         self._device = None     # CUDA device of the tree (set by load_cuda)
         self._data_loaded = False
         self._cuda_loaded = False
+        self._slot_map = False  # loaded with the table entry -> slot map (load_cuda(slot_map=True))
         if path is not None:
             self.open(path)
 
@@ -227,8 +228,11 @@ class N3Tree:
         self.ndc_height, self.ndc_width, self.ndc_focal = float(p[4]), float(p[9]), float(p[14])
 
     # -- device side (replaces src/cuda/n3tree.cu)
-    def load_cuda(self) -> None:
+    def load_cuda(self, slot_map: bool = False) -> None:
+        """Uploads the tree (vr_tree_create).  ``slot_map`` keeps the table entry -> slot map on the device
+        (VR_TREE_SLOT_MAP, 4 bytes per table entry), which :func:`leaf_weights` needs."""
         self.free_cuda()
+        flags = _capi.VR_TREE_SLOT_MAP if slot_map else 0
         use_quant = self.quant_ is not None and self.gpu_decode
         qd = _capi.vr_tree_quant_desc() if use_quant else None
         d = qd.base if use_quant else _capi.vr_tree_desc()
@@ -250,11 +254,12 @@ class N3Tree:
             qd.quant_colors, qd.quant_map, qd.sigma = q["colors"].ctypes.data, q["map"].ctypes.data, q["sigma"].ctypes.data
             qd.data_retained = q["retained"].ctypes.data if q["retained"] is not None else None
             qd.n_quant, qd.n_retain = q["n_quant"], q["n_retain"]
-            check(lib().vr_tree_create_quantized(C.byref(qd), C.byref(h)))
+            check(lib().vr_tree_create_quantized_ex(C.byref(qd), flags, C.byref(h)))
         else:
-            check(lib().vr_tree_create(C.byref(d), C.byref(h)))
+            check(lib().vr_tree_create_ex(C.byref(d), flags, C.byref(h)))
         self._handle = h
         self._cuda_loaded = True
+        self._slot_map = bool(slot_map)
         import torch
         self._device = torch.cuda.current_device()     # the device vr_tree_create put the tree on
 
@@ -278,6 +283,7 @@ class N3Tree:
             lib().vr_tree_destroy(self._handle)
             self._handle = None
         self._cuda_loaded = False
+        self._slot_map = False
 
     # -- grid wireframe (vr_tree_wireframe)
     def wireframe_vertex_count(self, max_depth: int = 100000) -> int:
@@ -629,6 +635,44 @@ def render_batch(tree: N3Tree, cams, options, images, *, float_out=None, counter
     oarr = _options_array(options)
     check(lib().vr_render_batch_opts(tree._handle, arr, len(cams), oarr, _rect(tile), img, fo, cn, s))
     _draw_probe_runs(tree, arr, options, oarr, tile, img, fo, s)
+
+
+def leaf_weights(tree: N3Tree, cams, options: RenderOptions, out=None, alpha=None, counters=None, stream=None, *,
+                 tile=None):
+    """Maximum compositing weight of every leaf slot over the views ``cams`` (vr_tree_leaf_weights): a CUDA float32
+    tensor ``[capacity, 2, 2, 2]`` (slot = node * 8 + octant) in which every shaded sample of every pixel has raised its
+    leaf's entry to at least its weight T * (1 - att).  ``out`` (same shape or ``capacity * 8`` elements, float32, on
+    the tree's device) accumulates over calls; without it a new tensor starts at -inf, the value of slots no view
+    shades.  ``options`` is one RenderOptions (step, thresholds and bbox act as in rendering).  ``alpha``: optional
+    float32 CUDA tensor ``[V, H, W]`` (tile-sized) that receives each ray's alpha; ``counters``: optional int64[5]
+    device tensor, accumulated.  Asynchronous on ``stream``.  The tree must be loaded with
+    ``load_cuda(slot_map=True)``."""
+    import torch
+    if not tree.is_cuda_loaded():
+        raise RuntimeError("N3Tree is not loaded on the device")
+    if not tree._slot_map:
+        raise RuntimeError("leaf_weights needs the slot map: load the tree with load_cuda(slot_map=True)")
+    if isinstance(cams, Camera):
+        cams = [cams]
+    if not isinstance(options, RenderOptions):
+        raise TypeError("leaf_weights takes one RenderOptions for every view")
+    dev = torch.device("cuda", tree._device)
+    n_slots = tree.capacity * tree.N ** 3
+    if out is None:
+        out = torch.full((tree.capacity, tree.N, tree.N, tree.N), float("-inf"), dtype=torch.float32, device=dev)
+    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
+          or not out.is_contiguous() or out.numel() != n_slots):
+        raise ValueError(f"out must be a contiguous float32 tensor of {n_slots} elements on {dev}")
+    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if cams else (0, 0)
+    if alpha is not None and (alpha.dtype != torch.float32 or alpha.device != dev or not alpha.is_contiguous()
+                              or alpha.numel() != len(cams) * w * h):
+        raise ValueError(f"alpha must be a contiguous float32 tensor of {len(cams)} x {h} x {w} elements on {dev}")
+    arr = _cams_array(cams)
+    o = options._as_c()
+    check(lib().vr_tree_leaf_weights(tree._handle, arr, len(cams), C.byref(o), _rect(tile), out.data_ptr(),
+                                     alpha.data_ptr() if alpha is not None else None,
+                                     counters.data_ptr() if counters is not None else None, _stream_ptr(stream)))
+    return out
 
 
 def _draw_probe_runs(tree: N3Tree, arr, options, oarr, tile, img, fo, s) -> None:
