@@ -215,8 +215,9 @@ def _draw_meshes(W, H, fx, fy, c2w12, meshes, rgba, depth):
     Returns (rgba, depth, winner) with winner = the winning z-buffer sequence number per pixel (0: none)."""
     fx, fy = F(fx), F(fy)
     c = np.asarray(c2w12, np.float32).reshape(12)
-    cam_pos = [c[9], c[10], c[11]]
     V = _w2c(c)
+    # camPos = -transpose(mat3(V)) * V[3] (mesh.cpp:376), in double as vr_draw_meshes_batch does
+    cam_pos = [F(-((V[0][k] * V[0][3] + V[1][k] * V[1][3]) + V[2][k] * V[2][3])) for k in range(3)]
     rgba = np.array(rgba, np.uint8, copy=True)
     depth = np.array(depth, np.float32, copy=True)
     key = (depth.view(np.uint32).astype(np.uint64) << np.uint64(32))

@@ -1331,7 +1331,10 @@ int vr_draw_meshes_batch(const vr_camera* cams, int n_views, const vr_mesh_desc*
         RasterFrame f{};
         f.W = W; f.H = H; f.fx = cam->fx; f.fy = cam->fy;
         f.cx = 0.5f * W; f.cy = 0.5f * H;
-        f.cam_pos[0] = c[9]; f.cam_pos[1] = c[10]; f.cam_pos[2] = c[11];
+        // camPos = -transpose(mat3(V)) * V[3] (mesh.cpp:376): the eye only when the rotation is orthonormal; a
+        // rotation scaled by s gives t / s^2
+        for (int k = 0; k < 3; ++k)
+            f.cam_pos[k] = (float)-((V[0][k] * V[0][3] + V[1][k] * V[1][3]) + V[2][k] * V[2][3]);
         f.rgba8 = rgba8_dev + (size_t)v * 4 * npx;
         f.depth = depth_dev + (size_t)v * npx;
         rf.push_back(f);

@@ -22,7 +22,7 @@ struct RasterMesh {
 struct RasterFrame {
     int W, H;
     float fx, fy, cx, cy;
-    float cam_pos[3];       // world camera position (the shader's camPos, mesh.cpp:376)
+    float cam_pos[3];       // the shader's camPos = -transpose(mat3(w2c)) * w2c[3] (mesh.cpp:376)
     long long large_off;    // this view's region of the large-primitive list (entries)
     uint8_t* rgba8;         // W * H * 4 bytes
     float* depth;           // W * H floats
