@@ -30,9 +30,13 @@ $(OBJ)/vr_kernels_%.o: volrend_b200/csrc/vr_kernels_inst.cu volrend_b200/csrc/vr
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -DVR_KBD=$* -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_$*.log || (cat $(OBJ)/ptxas_$*.log; false)
 
-$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h volrend_b200/csrc/vr_query.h include/volrend_b200.h
+$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_tree.h volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h volrend_b200/csrc/vr_query.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
+
+$(OBJ)/vr_tree.o: volrend_b200/csrc/vr_tree.cu volrend_b200/csrc/vr_tree.h volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_wire.h include/volrend_b200.h
+	@mkdir -p $(OBJ)
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_tree.log || (cat $(OBJ)/ptxas_tree.log; false)
 
 $(OBJ)/vr_raster.o: volrend_b200/csrc/vr_raster.cu volrend_b200/csrc/vr_raster.h
 	@mkdir -p $(OBJ)
@@ -66,7 +70,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp volrend_b200/csrc/vr_frames.h incl
 	@mkdir -p $(OBJ)
 	$(CXX) -O3 -std=c++17 -fPIC -Iinclude -c $< -o $@
 
-$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
+$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
 oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so

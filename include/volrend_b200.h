@@ -154,8 +154,7 @@ int vr_render_batch(const vr_tree* tree, const vr_camera* cams, int n_views, con
 /* Same, with options per view: view i is rendered with opts[i] (n_views entries), as vr_render would render it.
  * Output layout, tile, counters, the one-image-size rule and the splitting of very large batches are those of
  * vr_render_batch; NULL opts with n_views > 0 is VR_EINVAL.  The options travel through a device ring beside the
- * camera ring (allocated by the first such call on a (tree, stream)).  Batches of two or more views run on the
- * inline-shading (3 + 16*193) or shading-queue (7) kernel; any other vr_set_variant setting is VR_EUNSUPPORTED.
+ * camera ring (allocated by the first such call on a (tree, stream)).
  * Used by the animator (volrend_anim, main_anim.cpp:268-307), whose interpolated options change every frame. */
 int vr_render_batch_opts(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opts,
                          const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev,
@@ -185,8 +184,7 @@ int vr_render_composite(const vr_tree* tree, const vr_camera* cam, const vr_opti
 /* vr_render_composite for n_views views: view i's colour, depth limit and float output are the i-th tile-sized
  * frames of rgba8_dev, depth_dev and rgba32f_dev, and its bytes equal vr_render_composite of cams[i].  Tile, the
  * one-image-size rule and the splitting of very large batches are those of vr_render_batch; _opts renders view i
- * with opts[i].  Batches of two or more views run on the inline-shading (3 + 16*193) or shading-queue (7) kernel;
- * any other vr_set_variant setting is VR_EUNSUPPORTED. */
+ * with opts[i]. */
 int vr_render_composite_batch(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
                               const vr_rect* tile, uint8_t* rgba8_dev, const float* depth_dev, float* rgba32f_dev,
                               void* stream);
@@ -285,9 +283,6 @@ int vr_set_variant(int variant);
 int vr_get_variant(void);
 int vr_tree_variant(const vr_tree* tree);
 int vr_variant_supported(int kernel_basis, int variant);
-/* Cap the grid of the persistent march kernels at `max_ctas` CTAs (0 = all resident CTAs).  Used by
- * multi-GPU drivers to leave a few SMs to a concurrently running peer copy. */
-int vr_set_max_ctas(int max_ctas);
 /* Multi-GPU plumbing without SM-resident collectives: finished RGBA8 frames / bands are moved to the
  * gathering GPU by the copy engines over NVLink (cudaMemcpyAsync between peer-mapped buffers), so the
  * persistent march kernel keeps every SM.  vr_dev_alloc returns plain cudaMalloc memory (the base

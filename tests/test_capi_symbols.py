@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol(built):
         assert getattr(h, name) is not None, name
 
 
-def test_version_and_variant(built):
+def test_version_and_kernel_variants(built):
     from volrend_b200 import lib
     l = lib()
     assert b"sm_90a" in l.vr_version()
@@ -44,7 +44,6 @@ def test_version_and_variant(built):
         assert l.vr_variant_supported(kbd, 7) == 0 and l.vr_variant_supported(kbd, 3 + 16 * 193) == 1
     assert l.vr_variant_supported(16, 0) == 1 and l.vr_variant_supported(5, 0) == 0
     assert l.vr_set_variant(7) == 0 and l.vr_get_variant() == 7 and l.vr_set_variant(0) == 0
-    assert l.vr_set_max_ctas(-1) != 0 and l.vr_set_max_ctas(0) == 0
 
 
 def test_default_options_match_reference_defaults(built):

@@ -286,17 +286,6 @@ def test_composite_batch_variants_and_errors(built, trees):
     img = torch.zeros((2, 16, 16, 4), dtype=torch.uint8, device="cuda")
     dep = torch.full((2, 16, 16), 1e9, dtype=torch.float32, device="cuda")
     oarr = _options_array([RenderOptions(), RenderOptions()])
-    old = lib().vr_get_variant()
-    # a kernel other than the two product kernels, where the library has one (the experiment build does)
-    others = [v for v in range(1, 4096) if v not in (QUEUE, INLINE) and lib().vr_variant_supported(16, v)]
-    try:
-        for v in others[:1]:
-            assert lib().vr_set_variant(v) == 0
-            for fn in (lib().vr_render_composite_batch, lib().vr_render_composite_batch_opts):
-                assert fn(tree._handle, _cams_array(cams), 2, oarr, None, img.data_ptr(), dep.data_ptr(), None,
-                          None) == _capi.VR_EUNSUPPORTED
-    finally:
-        lib().vr_set_variant(old)
     for fn in (lib().vr_render_composite_batch, lib().vr_render_composite_batch_opts):
         assert fn(tree._handle, _cams_array(cams), 2, oarr, None, img.data_ptr(), None, None, None) == _capi.VR_EINVAL
         assert fn(tree._handle, _cams_array(cams), -1, oarr, None, img.data_ptr(), dep.data_ptr(), None,

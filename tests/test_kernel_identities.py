@@ -59,7 +59,7 @@ def test_in_cell_coordinate_with_rz_fma():
 
 
 def test_leaf_word_exponent_field():
-    # leaf entry of a wide table: 0x80000000 | (103 + depth) << 23 | sigma (vr_api.cu: build_wide_kernel)
+    # leaf entry of a wide table: 0x80000000 | (103 + depth) << 23 | sigma (vr_tree.cu: build_wide_kernel)
     for depth in range(1, 24):
         w = np.uint32(0x80000000 | ((103 + depth) << 23) | 0x3c00)
         cb = np.uint32(w & np.uint32(0x7f800000))

@@ -113,7 +113,6 @@ SYMBOLS = {
     "vr_get_variant": (C.c_int, []),
     "vr_tree_variant": (C.c_int, [C.c_void_p]),
     "vr_variant_supported": (C.c_int, [C.c_int, C.c_int]),
-    "vr_set_max_ctas": (C.c_int, [C.c_int]),
     "vr_dev_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p)]),
     "vr_dev_free": (C.c_int, [C.c_void_p]),
     "vr_ipc_export": (C.c_int, [C.c_void_p, C.c_char_p]),

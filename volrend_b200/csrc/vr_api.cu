@@ -1,28 +1,20 @@
 // vr_api.cu -- C-ABI of the H100 PlenOctree ray-marcher (declared in include/volrend_b200.h).
 //
-// Owns the device layout of a tree (the job of N3Tree::load_cuda, reference
-// src/cuda/n3tree.cu:9-41) and the launch logic (launch_renderer, src/cuda/volrend.cu:195-245).
+// Owns the launch logic (launch_renderer, reference src/cuda/volrend.cu:195-245) and the entry points; the device
+// layout of a tree (N3Tree::load_cuda) and vr_tree_create / vr_tree_destroy are in vr_tree.cu.
 // There is no CPU path in this library: every entry point needs a CUDA device.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
-#include <cub/device/device_scan.cuh>
-
 #include <algorithm>
-#include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <mutex>
 #include <string>
-#include <thread>
 #include <type_traits>
-#include <unordered_map>
 #include <vector>
 
-#include "volrend_b200.h"
 #include "vr_frames.h"
 #include "vr_kernels.h"
 #include "vr_normals.h"
@@ -30,17 +22,17 @@
 #include "vr_quant.h"
 #include "vr_query.h"
 #include "vr_raster.h"
-#include "vr_types.h"
+#include "vr_tree.h"
 #include "vr_wire.h"
 
 using namespace vrb;
 
 // ------------------------------------------------------------------------------------ errors
+std::atomic<unsigned long long> vrb::g_launches{0};
+
 namespace {
 thread_local std::string g_err;
 std::atomic<int> g_variant{0};
-std::atomic<unsigned long long> g_launches{0};
-std::atomic<int> g_max_ctas{0};
 constexpr int kQueueSlots = 256;
 constexpr int kCamRing = 8192;  // device ring of per-view cameras for batched launches
 }  // namespace
@@ -55,23 +47,21 @@ int vrb::fail(int code, const char* fmt, ...) {
     return code;
 }
 
-namespace {
-// A failed CUDA call: VR_ENOMEM for an allocation, else VR_ECUDA, with the message "<what>: <CUDA's text><where>".
-// The runtime's last error is cleared, so that a later launch check does not report this failure again.
-int cuda_fail(cudaError_t e, const char* what, const char* where = "") {
-    cudaGetLastError();
-    return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "%s: %s%s", what, cudaGetErrorString(e), where);
+int vrb::need_device(const vr_tree* t) {
+    int dev = -1, ndev = 0;
+    const bool ok = t ? cudaGetDevice(&dev) == cudaSuccess
+                      : cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && cudaGetDevice(&dev) == cudaSuccess;
+    if (!ok) {
+        cudaGetLastError();
+        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
+    }
+    if (t && dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
+    return VR_OK;
 }
-#define VR_STR_(x) #x
-#define VR_STR(x) VR_STR_(x)
-#define VR_CUDA(expr)                                                                                    \
-    do {                                                                                                 \
-        const cudaError_t e__ = (expr);                                                                  \
-        if (e__ != cudaSuccess) return cuda_fail(e__, #expr, " (" __FILE__ ":" VR_STR(__LINE__) ")"); \
-    } while (0)
 
-// f(std::integral_constant<int, K>{}) for the kernel bases K the march kernels are built for (vr_kernels_inst.cu, one
-// object per entry of the Makefile's KBDS); `otherwise` for any other kbd.
+namespace {
+// f(std::integral_constant<int, K>{}) for the kernel bases K the march kernels are built for (kbd_built); `otherwise`
+// for any other kbd.
 template <class R, class F>
 R with_kbd(int kbd, R otherwise, F f) {
     switch (kbd) {
@@ -84,13 +74,6 @@ R with_kbd(int kbd, R otherwise, F f) {
         default: return otherwise;
     }
 }
-
-int kernel_basis(int format, int basis_dim) {
-    if (format == VR_FMT_RGBA || basis_dim < 0) return -1;
-    // rt_core.cuh:134-160: no switch case matches -> only coefficient 0
-    return with_kbd(basis_dim, 1, [](auto k) { return decltype(k)::value; });
-}
-int rec_bytes_for(int kbd) { return kbd <= 1 ? 8 : ((3 * kbd * 2 + 15) / 16) * 16; }
 
 // All views of a batch have view 0's image size.
 int same_size(const vr_camera* cams, int n_views) {
@@ -112,65 +95,6 @@ int for_chunks(int n_views, int max_views, F f) {
 // p advanced by n elements; a null (absent) output stays null.
 template <class T>
 T* skip(T* p, size_t n) { return p ? p + n : p; }
-}  // namespace
-
-// Per-stream launch resources of a tree.  Work-queue slots and the camera ring are recycled in
-// stream order only: a launch that reuses a slot is ordered behind the launch that used it before, so
-// no fence is needed, and launches on different streams never share a slot.
-struct StreamRes {
-    unsigned int* queues = nullptr;  // kQueueSlots slots of kQueueSlotBytes: {head, done}, per-SM block states and locks (vr_march.cuh)
-    CamDev* cam_ring = nullptr;      // kCamRing entries; batches take consecutive slots
-    OptDev* opt_ring = nullptr;      // kCamRing entries beside cam_ring (same slots), allocated by the first
-                                     // batch with options per view
-    unsigned int next_queue = 0, cam_pos = 0;
-};
-
-struct vr_tree {
-    int device = 0;
-    int num_sms = 0;
-    TreeDev dev{};
-    uint32_t* wide = nullptr;
-    unsigned char* wrecs = nullptr;
-    float* extra = nullptr;
-    // upload scratch (slot-indexed node words, table entry -> slot), freed once the tables are built; with
-    // VR_TREE_SLOT_MAP the table entry -> slot map stays (vr_tree_leaf_weights)
-    uint32_t* nodes = nullptr;
-    uint32_t* wslot = nullptr;
-    long long n_tables = 0;
-    std::mutex res_mu;
-    std::unordered_map<cudaStream_t, StreamRes> res;
-    // vr_render_frames_host: chunk ring, streams and events are created once and kept
-    struct HostPath {
-        static constexpr int kRing = 4;
-        uint8_t* buf[kRing] = {};
-        size_t buf_bytes = 0;
-        cudaEvent_t rendered[kRing] = {}, copied[kRing] = {};
-        cudaStream_t sr[2] = {nullptr, nullptr}, sc = nullptr;
-        bool ready = false;
-    } host;
-    std::mutex host_mu;
-    vr_tree_info info{};
-    int data_dim = 0;
-    // grid wireframe (vr_tree_wireframe): cells per level, counted on the first call
-    std::mutex wire_mu;
-    bool wire_ready = false;
-    WireLevels wire_levels{};
-};
-
-namespace {
-// The device check of every entry point.  With a tree, the current device must be the tree's (cudaGetDevice only, so
-// launches pay no more); without one, some device must exist.
-int need_device(const vr_tree* t) {
-    int dev = -1, ndev = 0;
-    const bool ok = t ? cudaGetDevice(&dev) == cudaSuccess
-                      : cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && cudaGetDevice(&dev) == cudaSuccess;
-    if (!ok) {
-        cudaGetLastError();
-        return fail(VR_ENODEVICE, "no CUDA device: volrend_b200 has no CPU fallback");
-    }
-    if (t && dev != t->device) return fail(VR_EINVAL, "tree lives on device %d but device %d is current", t->device, dev);
-    return VR_OK;
-}
 
 // The tree's basis has no kernel of its own (kernel_basis): the device keeps only coefficient 0 of each channel.
 bool coef0_only(const vr_tree* t) { return t->dev.kbd > 0 && t->dev.kbd != t->dev.basis_dim; }
@@ -181,229 +105,6 @@ void basis_range(const vr_tree* t, const vr_options* opt, int32_t* bmin, int32_t
     const int nb = t->dev.kbd > 0 ? t->dev.kbd : 1;
     *bmin = opt ? std::max(opt->basis_minmax[0], 0) : 0;
     *bmax = opt ? std::min(opt->basis_minmax[1], nb - 1) : nb - 1;
-}
-}  // namespace
-
-// ------------------------------------------------------------------------------------ upload
-namespace {
-
-// Host -> device copy of a large pageable array at pinned-memory speed: a few worker threads copy
-// chunks into process-wide pinned staging buffers and issue the DMA from there (the reference uploads
-// with one synchronous pageable cudaMemcpy, src/cuda/n3tree.cu:20-33, ~12 GB/s).
-class Uploader {
-  public:
-    static constexpr int kWorkers = 4;
-    static constexpr size_t kChunk = 8u << 20;
-    static Uploader& get() { static Uploader u; return u; }
-    cudaError_t copy(void* dst, const void* src, size_t bytes) {
-        if (bytes < 4 * kChunk || !ensure()) return cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice);
-        std::lock_guard<std::mutex> lk(mu_);
-        int dev = 0;
-        cudaGetDevice(&dev);
-        const size_t n_chunks = (bytes + kChunk - 1) / kChunk;
-        std::atomic<int> err{0};
-        std::vector<std::thread> th;
-        for (int w = 0; w < kWorkers; ++w)
-            th.emplace_back([&, w]() {
-                cudaSetDevice(dev);
-                cudaStream_t st = nullptr;
-                cudaEvent_t ev[2] = {nullptr, nullptr};
-                if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) { err = 1; return; }
-                for (auto& e : ev) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-                int k = 0;
-                for (size_t c = (size_t)w; c < n_chunks && !err; c += kWorkers, ++k) {
-                    const size_t off = c * kChunk, n = bytes - off < kChunk ? bytes - off : kChunk;
-                    unsigned char* stage = stage_[2 * w + (k & 1)];
-                    if (k >= 2) cudaEventSynchronize(ev[k & 1]);   // the DMA that last read this buffer is done
-                    memcpy(stage, (const unsigned char*)src + off, n);
-                    if (cudaMemcpyAsync((unsigned char*)dst + off, stage, n, cudaMemcpyHostToDevice, st) != cudaSuccess) err = 1;
-                    cudaEventRecord(ev[k & 1], st);
-                }
-                if (cudaStreamSynchronize(st) != cudaSuccess) err = 1;
-                for (auto& e : ev) cudaEventDestroy(e);
-                cudaStreamDestroy(st);
-            });
-        for (auto& t : th) t.join();
-        return err ? cudaErrorUnknown : cudaSuccess;
-    }
-
-  private:
-    bool ensure() {
-        std::lock_guard<std::mutex> lk(mu_);
-        if (ready_) return true;
-        if (failed_) return false;
-        for (int i = 0; i < 2 * kWorkers; ++i)
-            if (cudaHostAlloc((void**)&stage_[i], kChunk, cudaHostAllocDefault) != cudaSuccess) {
-                cudaGetLastError();
-                failed_ = true;
-                return false;
-            }
-        ready_ = true;
-        return true;
-    }
-    std::mutex mu_;
-    unsigned char* stage_[2 * kWorkers] = {};
-    bool ready_ = false, failed_ = false;
-};
-
-}  // namespace
-
-// ------------------------------------------------------------------------------------ re-layout kernels
-namespace {
-
-// Source of the fp16 leaf data: the plain [slot][data_dim] array, or a quantised tree
-// (scripts/compress_octree.py; CPU decode in src/n3tree.cpp:309-340):
-//   data[slot][j + n_retain + k*n_total] = quant_colors[j][quant_map[j][slot]][k]   j < n_quant
-//   data[slot][j + k*n_total]            = data_retained[j][slot][k]                j < n_retain
-//   data[slot][data_dim-1]               = sigma[slot]
-struct LeafSrc {
-    const unsigned short* data;      // plain
-    const unsigned short* colors;    // quantised
-    const unsigned short* qmap;
-    const unsigned short* retained;
-    const unsigned short* sigma;
-    long long n_slots;
-    int data_dim, basis_dim, kbd, n_total, n_retain;
-};
-
-__device__ __forceinline__ unsigned short leaf_sigma(const LeafSrc& S, long long slot) {
-    return S.data ? S.data[(size_t)slot * S.data_dim + (S.data_dim - 1)] : S.sigma[slot];
-}
-
-// half c (= channel * kbd + j) of the padded colour record of `slot`
-__device__ __forceinline__ unsigned short leaf_half(const LeafSrc& S, long long slot, int c) {
-    if (S.kbd <= 1) {  // one coefficient per channel: RGBA -> halfs 0,1,2 ; basis -> k[0], k[bd], k[2bd]
-        if (c >= 3) return 0;
-        if (S.data) return S.data[(size_t)slot * S.data_dim + (S.kbd < 0 ? c : c * S.basis_dim)];
-        const int j = 0, k = c;  // quantised trees are never RGBA
-        if (j < S.n_retain) return S.retained[((size_t)j * S.n_slots + slot) * 3 + k];
-        return S.colors[((size_t)(j - S.n_retain) * 65536 + S.qmap[(size_t)(j - S.n_retain) * S.n_slots + slot]) * 3 + k];
-    }
-    if (c >= 3 * S.kbd) return 0;
-    if (S.data) return S.data[(size_t)slot * S.data_dim + c];
-    const int j = c % S.n_total, k = c / S.n_total;   // kbd == n_total here
-    if (j < S.n_retain) return S.retained[((size_t)j * S.n_slots + slot) * 3 + k];
-    const int q = j - S.n_retain;
-    return S.colors[((size_t)q * 65536 + S.qmap[(size_t)q * S.n_slots + slot]) * 3 + k];
-}
-
-// nodes[i]: absolute child id, or leaf bit | sigma.  Also validates child links.
-__global__ void relayout_nodes_kernel(const int32_t* __restrict__ child, LeafSrc S, uint32_t* __restrict__ nodes,
-                                      long long capacity, int* __restrict__ bad) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= S.n_slots) return;
-    const int32_t rel = child[i];
-    if (rel != 0) {
-        const long long tgt = (i >> 3) + rel;
-        if (tgt <= 0 || tgt >= capacity) {
-            atomicExch(bad, 1);
-            nodes[i] = kLeafBit;
-        } else {
-            nodes[i] = (uint32_t)tgt;
-        }
-    } else {
-        nodes[i] = kLeafBit | (uint32_t)leaf_sigma(S, i);
-    }
-}
-
-// depth[n] of every node by level-synchronous relaxation from the root.  A node that is reached
-// twice (two parents, or a cycle) makes the input a DAG, not a tree: rejected, because the table
-// builder and the ancestor stacks assume one depth per node.
-__global__ void node_depth_kernel(const uint32_t* __restrict__ nodes, int* __restrict__ depth, long long capacity,
-                                  int level, int* __restrict__ flags) {
-    const long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= capacity || depth[n] != level) return;
-#pragma unroll
-    for (int s = 0; s < 8; ++s) {
-        const uint32_t w = nodes[n * 8 + s];
-        if (!(w & kLeafBit)) {
-            if (atomicCAS(&depth[w], -1, level + 1) != -1) atomicExch(flags + 2, 1);
-            flags[1] = 1;
-        }
-    }
-}
-
-// cnt[r]: number of internal nodes whose depth is r modulo kWideLv
-__global__ void count_parity_kernel(const int* __restrict__ depth, long long capacity, unsigned long long* __restrict__ cnt) {
-    const long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int r = (n < capacity && depth[n] >= 0) ? depth[n] % kWideLv : -1;
-#pragma unroll
-    for (int k = 0; k < kWideLv; ++k) {
-        const unsigned int c = __reduce_add_sync(0xffffffffu, r == k ? 1u : 0u);
-        if ((threadIdx.x & 31) == 0 && c) atomicAdd(cnt + k, (unsigned long long)c);
-    }
-}
-
-// a node owns a table when it is the root or its depth d has (d + v) % kWideLv == 0
-__global__ void table_flag_kernel(const int* __restrict__ depth, long long capacity, int v, uint32_t* __restrict__ flag) {
-    const long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= capacity) return;
-    const int d = depth[n];
-    flag[n] = (d >= 0 && (n == 0 || (d + v) % kWideLv == 0)) ? 1u : 0u;
-}
-
-// wide[table * E + e], E = 8^kWideLv: e = ex << 2*LV | ey << LV | ez holds kWideLv octree levels per axis, first level
-// in the high bit.  The tree hangs v levels below a virtual root (octant 0 each time), so the root table resolves only
-// kWideLv - v real levels: its entries with a non-zero virtual bit are never looked up.
-__global__ void build_wide_kernel(const uint32_t* __restrict__ nodes, const int* __restrict__ depth,
-                                  const uint32_t* __restrict__ tid, uint32_t* __restrict__ wide,
-                                  uint32_t* __restrict__ wslot, long long capacity, int v) {
-    constexpr int LV = kWideLv, M = (1 << LV) - 1;
-    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long n = g >> (3 * LV);
-    const int e = (int)(g & (kWideEntries - 1));
-    if (n >= capacity) return;
-    const int d = depth[n];
-    if (d < 0 || (n != 0 && (d + v) % LV != 0)) return;   // unreachable, or folded into an ancestor's table
-    // leaf entry = kLeafBit | (103 + leaf depth + v) << 23 | sigma: the exponent field of the cube size on the
-    // 2^(24-v) position grid (vr_march.cuh)
-    const uint32_t ex = (e >> (2 * LV)) & M, ey = (e >> LV) & M, ez = e & M;
-    const size_t o = (size_t)tid[n] * kWideEntries + e;
-    uint32_t node = (uint32_t)n;
-    int dn = d;
-    for (int k = (n == 0) ? v : 0; k < LV; ++k) {
-        const int sh = LV - 1 - k;
-        const uint32_t oct = (((ex >> sh) & 1u) << 2) | (((ey >> sh) & 1u) << 1) | ((ez >> sh) & 1u);
-        const uint32_t s = node * 8u + oct;
-        const uint32_t w = nodes[s];
-        if (w & kLeafBit) {
-            wide[o] = kLeafBit | ((uint32_t)(103 + dn + 1 + v) << 23) | (w & 0xffffu);
-            wslot[o] = s;
-            return;
-        }
-        node = w;
-        ++dn;
-    }
-    wide[o] = tid[node];
-    wslot[o] = 0xffffffffu;
-}
-
-// wrecs[entry]: padded colour record of the entry's leaf, straight from the source arrays
-// (16-byte chunks; 8-byte records as one chunk).  Entries that are not leaves stay zero.
-__global__ void build_wrecs_kernel(const uint32_t* __restrict__ wslot, LeafSrc S, unsigned char* __restrict__ wrecs,
-                                   long long n_entries, int rec_bytes) {
-    const int chunks = rec_bytes >= 16 ? rec_bytes / 16 : 1;
-    const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long e = gid / chunks;
-    const int c = (int)(gid % chunks);
-    if (e >= n_entries) return;
-    const uint32_t slot = wslot[e];
-    const bool leaf = slot != 0xffffffffu;
-    if (rec_bytes == 8) {
-        ushort4 v = make_ushort4(0, 0, 0, 0);
-        if (leaf) { v.x = leaf_half(S, slot, 0); v.y = leaf_half(S, slot, 1); v.z = leaf_half(S, slot, 2); }
-        reinterpret_cast<ushort4*>(wrecs)[e] = v;
-        return;
-    }
-    unsigned short h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    if (leaf) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) h[j] = leaf_half(S, slot, c * 8 + j);
-    }
-    uint4 v;
-    v.x = h[0] | ((uint32_t)h[1] << 16); v.y = h[2] | ((uint32_t)h[3] << 16);
-    v.z = h[4] | ((uint32_t)h[5] << 16); v.w = h[6] | ((uint32_t)h[7] << 16);
-    reinterpret_cast<uint4*>(wrecs + (size_t)e * rec_bytes)[c] = v;
 }
 
 // one block per queue slot: {head, done} = 0, every SM's block state = "no block", locks free (vr_march.cuh next_item)
@@ -416,277 +117,6 @@ __global__ void queue_init_kernel(unsigned char* slots) {
 }
 
 }  // namespace
-
-// ------------------------------------------------------------------------------------ C-ABI
-extern "C" {
-
-const char* vr_last_error(void) { return g_err.c_str(); }
-const char* vr_version(void) { return "volrend_b200 0.2 (sm_90a)"; }
-static bool variant_ok(int kbd, int variant) {
-    return with_kbd(kbd, false, [&](auto k) { return variant_supported<decltype(k)::value>(variant); });
-}
-int vr_variant_supported(int kernel_basis, int variant) { return variant >= 0 && variant_ok(kernel_basis, variant) ? 1 : 0; }
-int vr_set_variant(int variant) {
-    // accepted when at least one basis size has it; a tree whose basis size lacks it fails at launch
-    bool any = false;
-    for (int kbd = -1; kbd <= VR_BASIS_MAX; ++kbd) any = any || (variant >= 0 && variant_ok(kbd, variant));
-    if (!any) return fail(VR_EINVAL, "kernel variant %d is not built into this library", variant);
-    g_variant.store(variant);
-    return VR_OK;
-}
-int vr_get_variant(void) { return g_variant.load(); }
-int vr_set_max_ctas(int max_ctas) {
-    if (max_ctas < 0) return fail(VR_EINVAL, "max_ctas < 0");
-    g_max_ctas.store(max_ctas);
-    return VR_OK;
-}
-int vr_tree_variant(const vr_tree* t) {
-    if (!t) return -1;
-    const int v = g_variant.load();
-    if (v != 0) return variant_ok(t->dev.kbd, v) ? v : -1;
-    return kVariantInline;
-}
-unsigned long long vr_launch_count(void) { return g_launches.load(); }
-
-void vr_default_options(vr_options* o) {
-    if (!o) return;
-    memset(o, 0, sizeof(*o));
-    o->step_size = 1e-4f; o->sigma_thresh = 1e-2f; o->stop_thresh = 1e-2f;  // render_options.hpp:14-23
-    o->background_brightness = 1.f;
-    o->render_bbox[3] = o->render_bbox[4] = o->render_bbox[5] = 1.f;
-    o->basis_minmax[0] = 0; o->basis_minmax[1] = VR_BASIS_MAX - 1;
-}
-
-void vr_tree_destroy(vr_tree* t) {
-    if (!t) return;
-    int prev = 0;
-    cudaGetDevice(&prev);
-    cudaSetDevice(t->device);
-    cudaFree(t->nodes); cudaFree(t->extra);
-    cudaFree(t->wide); cudaFree(t->wslot); cudaFree(t->wrecs);
-    for (auto& kv : t->res) { cudaFree(kv.second.queues); cudaFree(kv.second.cam_ring); cudaFree(kv.second.opt_ring); }
-    for (int i = 0; i < vr_tree::HostPath::kRing; ++i) {
-        cudaFree(t->host.buf[i]);
-        if (t->host.rendered[i]) cudaEventDestroy(t->host.rendered[i]);
-        if (t->host.copied[i]) cudaEventDestroy(t->host.copied[i]);
-    }
-    for (auto st : t->host.sr) if (st) cudaStreamDestroy(st);
-    if (t->host.sc) cudaStreamDestroy(t->host.sc);
-    cudaSetDevice(prev);
-    delete t;
-}
-
-static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, uint32_t create_flags, vr_tree** out) {
-    if (!d || !out) return fail(VR_EINVAL, "null argument");
-    *out = nullptr;
-    if (create_flags & ~(uint32_t)VR_TREE_SLOT_MAP) return fail(VR_EINVAL, "unknown tree flags 0x%x", create_flags);
-    if (int rc = need_device(nullptr)) return rc;
-    if (d->N != 2) return fail(VR_EUNSUPPORTED, "N=%d: only N=2 octrees are supported (as in the reference)", d->N);
-    if (d->capacity < 1 || d->capacity >= (1ll << 28)) return fail(VR_EINVAL, "capacity %lld out of range", (long long)d->capacity);
-    if (!d->child || (!q && !d->data)) return fail(VR_EINVAL, "child/data arrays missing");
-    if (q) {
-        if (!q->quant_colors || !q->quant_map || !q->sigma) return fail(VR_EINVAL, "quantised arrays missing");
-        if (q->n_quant < 1 || q->n_retain < 0 || (q->n_retain > 0 && !q->data_retained))
-            return fail(VR_EINVAL, "bad quantised basis counts");
-        if (d->format == VR_FMT_RGBA || q->n_quant + q->n_retain != d->basis_dim)
-            return fail(VR_EINVAL, "codebook and map basis numbers does not match");   // n3tree.cpp:296-299
-    }
-    if (d->format < VR_FMT_RGBA || d->format > VR_FMT_ASG) return fail(VR_EINVAL, "bad data format %d", d->format);
-    const int kbd = kernel_basis(d->format, d->basis_dim);
-    if (kbd < 0 ? d->data_dim < 4 : d->data_dim < 3 * d->basis_dim + 1)
-        return fail(VR_EINVAL, "data_dim %d too small for format %d basis %d", d->data_dim, d->format, d->basis_dim);
-    if ((d->format == VR_FMT_SG || d->format == VR_FMT_ASG) && !d->extra)
-        return fail(VR_EINVAL, "SG/ASG trees need extra_data");
-    if ((d->format == VR_FMT_SG || d->format == VR_FMT_ASG) && d->basis_dim > VR_BASIS_MAX)
-        return fail(VR_EINVAL, "basis_dim %d > %d", d->basis_dim, VR_BASIS_MAX);
-
-    vr_tree* t = new vr_tree();
-    struct Guard { vr_tree*& t; bool ok = false; ~Guard() { if (!ok) { vr_tree_destroy(t); t = nullptr; } } } guard{t};
-    VR_CUDA(cudaGetDevice(&t->device));
-    cudaDeviceProp prop;
-    VR_CUDA(cudaGetDeviceProperties(&prop, t->device));
-    t->num_sms = prop.multiProcessorCount;
-    t->data_dim = d->data_dim;
-    const long long n_slots = d->capacity * 8;
-    const int rec_bytes = rec_bytes_for(kbd);
-    const int TB = 256;
-    Uploader& up = Uploader::get();
-
-    // device scratch, freed on every exit path
-    std::vector<void*> scratch;
-    struct Scratch { std::vector<void*>& v; ~Scratch() { for (void* p : v) cudaFree(p); } } scratch_guard{scratch};
-    auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
-        cudaError_t e = cudaMalloc(p, bytes ? bytes : 1);
-        if (e == cudaSuccess) scratch.push_back(*p);
-        return e;
-    };
-    auto release = [&](void* p) {
-        for (auto& s : scratch) if (s == p) { cudaFree(p); s = nullptr; }
-    };
-
-    int32_t* raw_child = nullptr;
-    int* flags = nullptr;   // {bad link, changed, node reached twice}
-    int* depth = nullptr;
-    LeafSrc S{};
-    S.n_slots = n_slots; S.data_dim = d->data_dim; S.basis_dim = d->basis_dim; S.kbd = kbd;
-    S.n_total = d->basis_dim; S.n_retain = q ? q->n_retain : 0;
-    VR_CUDA(dalloc((void**)&raw_child, (size_t)n_slots * 4));
-    VR_CUDA(dalloc((void**)&flags, 4 * sizeof(int)));
-    VR_CUDA(dalloc((void**)&depth, (size_t)d->capacity * sizeof(int)));
-    VR_CUDA(cudaMalloc(&t->nodes, (size_t)n_slots * 4));
-    VR_CUDA(up.copy(raw_child, d->child, (size_t)n_slots * 4));
-    if (!q) {
-        unsigned short* raw = nullptr;
-        const size_t data_bytes = (size_t)n_slots * d->data_dim * 2;
-        VR_CUDA(dalloc((void**)&raw, data_bytes));
-        VR_CUDA(up.copy(raw, d->data, data_bytes));
-        S.data = raw;
-    } else {
-        const size_t cb = (size_t)q->n_quant * 65536 * 3 * 2, mb = (size_t)q->n_quant * n_slots * 2,
-                     sb = (size_t)n_slots * 2, rb = (size_t)q->n_retain * n_slots * 3 * 2;
-        unsigned short *qc = nullptr, *qm = nullptr, *qs = nullptr, *qr = nullptr;
-        VR_CUDA(dalloc((void**)&qc, cb));
-        VR_CUDA(dalloc((void**)&qm, mb));
-        VR_CUDA(dalloc((void**)&qs, sb));
-        VR_CUDA(up.copy(qc, q->quant_colors, cb));
-        VR_CUDA(up.copy(qm, q->quant_map, mb));
-        VR_CUDA(up.copy(qs, q->sigma, sb));
-        if (q->n_retain > 0) {
-            VR_CUDA(dalloc((void**)&qr, rb));
-            VR_CUDA(up.copy(qr, q->data_retained, rb));
-        }
-        S.colors = qc; S.qmap = qm; S.sigma = qs; S.retained = qr;
-    }
-    VR_CUDA(cudaMemset(flags, 0, 4 * sizeof(int)));
-    if (d->extra && (d->format == VR_FMT_SG || d->format == VR_FMT_ASG)) {
-        const size_t nf = (size_t)d->basis_dim * (d->format == VR_FMT_SG ? 4 : 11);
-        VR_CUDA(cudaMalloc(&t->extra, nf * sizeof(float)));
-        VR_CUDA(cudaMemcpy(t->extra, d->extra, nf * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    relayout_nodes_kernel<<<(unsigned)((n_slots + TB - 1) / TB), TB>>>(raw_child, S, t->nodes, d->capacity, flags);
-    VR_CUDA(cudaGetLastError());
-    release(raw_child);
-
-    // node depths (level-synchronous sweep) -> max leaf depth; validates that the links form a tree
-    VR_CUDA(cudaMemset(depth, 0xff, (size_t)d->capacity * sizeof(int)));
-    VR_CUDA(cudaMemset(depth, 0, sizeof(int)));
-    int max_node_depth = 0;
-    int h_flags[3] = {0, 0, 0};
-    for (int level = 0;; ++level) {
-        if (level >= kMaxTreeDepth) return fail(VR_EUNSUPPORTED, "tree deeper than %d levels (or its child links form a cycle)", kMaxTreeDepth);
-        VR_CUDA(cudaMemsetAsync(flags + 1, 0, sizeof(int)));
-        node_depth_kernel<<<(unsigned)((d->capacity + TB - 1) / TB), TB>>>(t->nodes, depth, d->capacity, level, flags);
-        VR_CUDA(cudaMemcpy(h_flags, flags, sizeof(h_flags), cudaMemcpyDeviceToHost));
-        if (h_flags[0]) return fail(VR_EINVAL, "child array has links outside [1, capacity)");
-        if (h_flags[2]) return fail(VR_EINVAL, "child array is not a tree: a node is reachable along two paths");
-        if (!h_flags[1]) break;
-        max_node_depth = level + 1;
-    }
-
-    // kWideLv-levels-per-step tables.  Which nodes own one: those whose depth d has (d + v) % kWideLv == 0, plus the
-    // root; the v with the fewest tables wins -- with another one every table at the deepest internal level would
-    // replicate its 8 leaves 8 (or 64) times (several times more colour-record memory).
-    unsigned long long* pcnt = nullptr;
-    VR_CUDA(dalloc((void**)&pcnt, 4 * sizeof(unsigned long long)));
-    VR_CUDA(cudaMemset(pcnt, 0, 4 * sizeof(unsigned long long)));
-    count_parity_kernel<<<(unsigned)((d->capacity + TB - 1) / TB), TB>>>(depth, d->capacity, pcnt);
-    unsigned long long h_pcnt[4] = {0, 0, 0, 0};
-    VR_CUDA(cudaMemcpy(h_pcnt, pcnt, sizeof(h_pcnt), cudaMemcpyDeviceToHost));
-    int wp = 0;
-    unsigned long long n_tab64 = ~0ull;
-    for (int v = 0; v < kWideLv; ++v) {
-        if (max_node_depth + 1 + v > 24) continue;   // leaf depth + v must fit the 24-bit position grid
-        const unsigned long long nt = h_pcnt[(kWideLv - v) % kWideLv] + (v ? 1 : 0);
-        if (nt + 1 < n_tab64 || n_tab64 == ~0ull) { n_tab64 = nt; wp = v; }
-    }
-    if (const char* e = getenv("VR_WIDE_PARITY")) {
-        const int v = atoi(e);
-        if (v >= 0 && v < kWideLv && max_node_depth + 1 + v <= 24) { wp = v; n_tab64 = h_pcnt[(kWideLv - v) % kWideLv] + (v ? 1 : 0); }
-    }
-    if (n_tab64 * (unsigned long long)kWideEntries >= (1ull << 32)) return fail(VR_EUNSUPPORTED, "too many nodes for the wide tables");
-    const uint32_t n_tab = (uint32_t)n_tab64;
-    const long long n_entries = (long long)n_tab * kWideEntries;
-    {
-        uint32_t *flag = nullptr, *tid = nullptr;
-        void* tmp = nullptr;
-        size_t tmp_bytes = 0;
-        VR_CUDA(dalloc((void**)&flag, (size_t)d->capacity * 4));
-        VR_CUDA(dalloc((void**)&tid, (size_t)d->capacity * 4));
-        table_flag_kernel<<<(unsigned)((d->capacity + TB - 1) / TB), TB>>>(depth, d->capacity, wp, flag);
-        VR_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flag, tid, (int)d->capacity));
-        VR_CUDA(dalloc(&tmp, tmp_bytes));
-        VR_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, tid, (int)d->capacity));
-        VR_CUDA(cudaMalloc(&t->wide, (size_t)n_entries * 4));
-        VR_CUDA(cudaMalloc(&t->wslot, (size_t)n_entries * 4));
-        const long long work = d->capacity * (long long)kWideEntries;
-        build_wide_kernel<<<(unsigned)((work + TB - 1) / TB), TB>>>(t->nodes, depth, tid, t->wide, t->wslot, d->capacity, wp);
-        VR_CUDA(cudaGetLastError());
-        release(flag); release(tid); release(tmp);
-    }
-    release(depth);
-    {
-        const size_t wrec_bytes = (size_t)n_entries * rec_bytes;
-        const cudaError_t e = cudaMalloc(&t->wrecs, wrec_bytes);
-        if (e != cudaSuccess) {
-            char what[128];
-            snprintf(what, sizeof(what), "colour records of the wide tables need %.2f GB (%lld entries x %d B)",
-                     wrec_bytes / 1e9, n_entries, rec_bytes);
-            return cuda_fail(e, what);
-        }
-        const long long rwork = n_entries * (rec_bytes >= 16 ? rec_bytes / 16 : 1);
-        build_wrecs_kernel<<<(unsigned)((rwork + TB - 1) / TB), TB>>>(t->wslot, S, t->wrecs, n_entries, rec_bytes);
-        VR_CUDA(cudaGetLastError());
-    }
-    VR_CUDA(cudaDeviceSynchronize());
-    // the march kernels read the tables and the table-indexed records only; the weights pass also the slot map
-    cudaFree(t->nodes); t->nodes = nullptr;
-    const bool slot_map = (create_flags & VR_TREE_SLOT_MAP) != 0;
-    if (!slot_map) { cudaFree(t->wslot); t->wslot = nullptr; }
-    t->n_tables = n_tab;
-    g_launches += 7;
-
-    TreeDev& D = t->dev;
-    D.wide = t->wide; D.wrecs = t->wrecs; D.extra = t->extra;
-    for (int i = 0; i < 3; ++i) { D.offset[i] = d->offset[i]; D.scale[i] = d->scale[i]; }
-    D.ndc_width = d->use_ndc ? d->ndc_width : -1.f;  // data_spec.hpp:47
-    D.ndc_height = d->ndc_height; D.ndc_focal = d->ndc_focal;
-    D.N = d->N; D.format = d->format; D.basis_dim = d->basis_dim; D.kbd = kbd;
-    D.rec_bytes = rec_bytes; D.max_depth = max_node_depth + 1; D.wide_p = wp; D.wide_entries = (uint32_t)n_entries;
-    D.pos_scale = (float)(1u << (24 - wp));
-    D.pos_hi = (1.f - 1e-6f) * D.pos_scale;   // exact: a power-of-two multiple of 0x3F7FFFEF
-    D.icube_bias = 0x73000000u + ((uint32_t)wp << 23);
-    vr_tree_info& I = t->info;
-    I.capacity = d->capacity; I.max_depth = D.max_depth; I.rec_bytes = rec_bytes;
-    I.node_bytes = n_slots * 4; I.rec_total_bytes = n_slots * (long long)rec_bytes;
-    I.top_bytes = 16 * 16 * 16 * 4;   // a dense 16^3 grid of node words
-    I.kernel_basis = kbd; I.wide_parity = wp; I.n_tables = n_tab;
-    I.wide_bytes = n_entries * 4; I.wrecs_bytes = n_entries * (long long)rec_bytes;
-    I.kernel_bytes = I.wide_bytes + I.wrecs_bytes;
-    I.device_bytes = I.kernel_bytes + (slot_map ? n_entries * 4 : 0);
-    guard.ok = true;
-    *out = t;
-    return VR_OK;
-}
-
-int vr_tree_create_ex(const vr_tree_desc* d, uint32_t flags, vr_tree** out) {
-    return tree_create_impl(d, nullptr, flags, out);
-}
-int vr_tree_create(const vr_tree_desc* d, vr_tree** out) { return vr_tree_create_ex(d, 0, out); }
-
-int vr_tree_create_quantized_ex(const vr_tree_quant_desc* q, uint32_t flags, vr_tree** out) {
-    if (!q) return fail(VR_EINVAL, "null argument");
-    if (q->base.data) return fail(VR_EINVAL, "quantised descriptor must not carry decoded data");
-    return tree_create_impl(&q->base, q, flags, out);
-}
-int vr_tree_create_quantized(const vr_tree_quant_desc* q, vr_tree** out) { return vr_tree_create_quantized_ex(q, 0, out); }
-
-int vr_tree_get_info(const vr_tree* t, vr_tree_info* info) {
-    if (!t || !info) return fail(VR_EINVAL, "null argument");
-    *info = t->info;
-    return VR_OK;
-}
-
-}  // extern "C"
 
 // ------------------------------------------------------------------------------------ launch plumbing
 namespace {
@@ -727,22 +157,24 @@ int stream_res(vr_tree* t, cudaStream_t stream, StreamRes*& out) {
     return VR_OK;
 }
 
-// weights: the weights pass (one kernel for every basis size, whatever the variant setting)
+// One launch of P.n_views views, on the kernel march_kernel() picks.  weights: the weights pass (one kernel for every
+// basis size, whatever the variant setting).
 int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStream_t stream, bool weights = false) {
+    const int variant = vr_get_variant();
+    const MarchKernel kernel = march_kernel(t->dev.kbd, variant, P.n_views);
+    if (!weights && kernel == MarchKernel::kNotBuilt)
+        return fail(VR_EUNSUPPORTED, "kernel variant %d is not available for kernel basis %d", variant, t->dev.kbd);
     LaunchCfg cfg;
-    cfg.variant = vr_get_variant();
-    if (!weights && !variant_ok(t->dev.kbd, cfg.variant))
-        return fail(VR_EUNSUPPORTED, "kernel variant %d is not available for kernel basis %d", cfg.variant, t->dev.kbd);
-    cfg.max_ctas = g_max_ctas.load();
+    cfg.queue = kernel == MarchKernel::kQueue;
     cfg.count = count; cfg.surface = surface; cfg.num_sms = t->num_sms; cfg.stream = stream;
     vr_tree* mt = const_cast<vr_tree*>(t);
     StreamRes* sr = nullptr;
     if (int rc = stream_res(mt, stream, sr)) return rc;
     {
         std::lock_guard<std::mutex> lk(mt->res_mu);
-        cfg.queue = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(sr->queues) + (size_t)(sr->next_queue++ % kQueueSlots) * kQueueSlotBytes);
+        cfg.work_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(sr->queues) + (size_t)(sr->next_queue++ % kQueueSlots) * kQueueSlotBytes);
     }
-    // variant_ok above has rejected every kbd without kernels
+    // march_kernel above has rejected every kbd without kernels
     const cudaError_t e = weights ? launch_weights(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
         return launch_march<decltype(k)::value>(P, cfg);
     });
@@ -768,6 +200,17 @@ int check_common(const vr_tree* t, const vr_camera* cam, const vr_options* opt, 
     if (tile_bound(r) > 0x7fffffffLL)
         return fail(VR_EUNSUPPORTED, "%dx%d pixels: more tiles than the 31-bit work queue can index", r.w, r.h);
     return need_device(t);
+}
+
+// The opening checks of the batch entry points: n_views >= 0, and for a non-empty batch check_common (r: the tile or
+// the full frame of view 0) and one image size for every view.  An empty batch is VR_OK before any pointer is read;
+// callers return once it is checked.
+int check_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, const vr_rect* tile,
+                vr_rect& r) {
+    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
+    if (n_views == 0) return VR_OK;
+    if (int rc = check_common(t, cams, opt, tile, r)) return rc;
+    return same_size(cams, n_views);
 }
 
 // Cameras of a batch go through a device ring owned by (tree, stream): no allocation on the launch path (a
@@ -840,28 +283,15 @@ int render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views,
 }
 }  // namespace
 
-namespace vrb {
-
 // vr_render_batch (opt_stride 0: one options struct for every view) and vr_render_batch_opts (opt_stride 1: view i
 // uses opt[i]).
-int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
-                 const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream,
-                 const float* depth_dev) {
-    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
-    if (n_views == 0) return VR_OK;
+int vrb::render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
+                      const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev,
+                      void* stream, const float* depth_dev) {
     vr_rect r;
-    int rc = check_common(t, cams, opt, tile, r);
-    if (rc) return rc;
-    if ((rc = same_size(cams, n_views))) return rc;
+    const int rc = check_batch(t, cams, n_views, opt, tile, r);
+    if (rc || n_views == 0) return rc;
     if (depth_dev && !rgba8_dev) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
-    const bool per_view = opt_stride != 0 && n_views > 1;
-    if ((per_view || depth_dev) && n_views > 1) {
-        // per-view options and composite batches are checked on the two product kernels (inline shading, shading
-        // queue) only
-        const int v = vr_get_variant();
-        if (v != 0 && v != kVariantQueue && v != kVariantInline)
-            return fail(VR_EUNSUPPORTED, "kernel variant %d has no per-view options or composite batch form", v);
-    }
     if (r.w == 0 || r.h == 0) return VR_OK;
     LaunchDev P{};
     P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
@@ -871,9 +301,36 @@ int render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_
     return march(t, cams, n_views, opt, opt_stride, P, false, (cudaStream_t)stream);
 }
 
-}  // namespace vrb
-
+// ------------------------------------------------------------------------------------ C-ABI
 extern "C" {
+
+const char* vr_last_error(void) { return g_err.c_str(); }
+const char* vr_version(void) { return "volrend_b200 0.2 (sm_90a)"; }
+int vr_variant_supported(int kernel_basis, int variant) {
+    return march_kernel(kernel_basis, variant, 1) != MarchKernel::kNotBuilt ? 1 : 0;
+}
+int vr_set_variant(int variant) {
+    // accepted when at least one basis size has it; a tree whose basis size lacks it fails at launch
+    for (int kbd = -1; kbd <= VR_BASIS_MAX; ++kbd)
+        if (vr_variant_supported(kbd, variant)) { g_variant.store(variant); return VR_OK; }
+    return fail(VR_EINVAL, "kernel variant %d is not built into this library", variant);
+}
+int vr_get_variant(void) { return g_variant.load(); }
+int vr_tree_variant(const vr_tree* t) {
+    if (!t) return -1;
+    const MarchKernel k = march_kernel(t->dev.kbd, g_variant.load(), 2);   // two views: a batch
+    return k == MarchKernel::kQueue ? kVariantQueue : k == MarchKernel::kInline ? kVariantInline : -1;
+}
+unsigned long long vr_launch_count(void) { return g_launches.load(); }
+
+void vr_default_options(vr_options* o) {
+    if (!o) return;
+    memset(o, 0, sizeof(*o));
+    o->step_size = 1e-4f; o->sigma_thresh = 1e-2f; o->stop_thresh = 1e-2f;  // render_options.hpp:14-23
+    o->background_brightness = 1.f;
+    o->render_bbox[3] = o->render_bbox[4] = o->render_bbox[5] = 1.f;
+    o->basis_minmax[0] = 0; o->basis_minmax[1] = VR_BASIS_MAX - 1;
+}
 
 int vr_render_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, const vr_rect* tile,
                     uint8_t* rgba8_dev, float* rgba32f_dev, vr_counters* counters_dev, void* stream) {
@@ -889,13 +346,10 @@ int vr_render_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, c
 int vr_tree_leaf_weights(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
                          const vr_rect* tile, float* weight_dev, float* alpha_dev, vr_counters* counters_dev,
                          void* stream) {
-    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
-    if (n_views == 0) return VR_OK;
-    if (!weight_dev) return fail(VR_EINVAL, "null weight buffer");
+    if (n_views > 0 && !weight_dev) return fail(VR_EINVAL, "null weight buffer");
     vr_rect r;
-    int rc = check_common(t, cams, opt, tile, r);
-    if (rc) return rc;
-    if ((rc = same_size(cams, n_views))) return rc;
+    const int rc = check_batch(t, cams, n_views, opt, tile, r);
+    if (rc || n_views == 0) return rc;
     if (!t->wslot)
         return fail(VR_EUNSUPPORTED, "leaf weights need the slot map: create the tree with VR_TREE_SLOT_MAP");
     if (r.w == 0 || r.h == 0) return VR_OK;
@@ -920,14 +374,11 @@ int vr_render_composite_batch_opts(const vr_tree* t, const vr_camera* cams, int 
 
 int vr_render_bands_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int band_h,
                           int n_parts, int part, uint8_t* rgba8_dev, float* rgba32f_dev, void* stream) {
-    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
-    if (n_views == 0) return VR_OK;
     vr_rect r;
-    int rc = check_common(t, cams, opt, nullptr, r);
-    if (rc) return rc;
+    const int rc = check_batch(t, cams, n_views, opt, nullptr, r);
+    if (rc || n_views == 0) return rc;
     if (band_h < 4 || band_h % 4 || n_parts < 1 || part < 0 || part >= n_parts)
         return fail(VR_EINVAL, "bands: band_h must be a positive multiple of 4 and 0 <= part < n_parts");
-    if ((rc = same_size(cams, n_views))) return rc;
     const int rows = vr_band_rows(cams[0].height, band_h, n_parts, part);
     if (rows == 0) return VR_OK;
     LaunchDev P{};
@@ -996,17 +447,12 @@ int vrb::render_frames_host(const vr_tree* t, const vr_camera* cams, int n_views
     // rendered in chunks of a few views per launch on two alternating streams (the tail of
     // one chunk overlaps the head of the next) and copied out on a third stream while the
     // following chunks render.
-    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
-    if (n_views == 0) return VR_OK;
-    if (!rgba8_host) return fail(VR_EINVAL, "null host buffer");
+    if (n_views > 0 && !rgba8_host) return fail(VR_EINVAL, "null host buffer");
     vr_rect r;
-    int rc = check_common(t, cams, opt, nullptr, r);
-    if (rc) return rc;
-    if ((rc = same_size(cams, n_views))) return rc;
+    int rc = check_batch(t, cams, n_views, opt, nullptr, r);
+    if (rc || n_views == 0) return rc;
     const size_t frame = (size_t)4 * r.w * r.h;
-    int chunk = 8;
-    if (const char* e = getenv("VR_HOST_CHUNK")) chunk = atoi(e) > 0 ? atoi(e) : chunk;
-    if (chunk > n_views) chunk = n_views;
+    const int chunk = std::min(8, n_views);
     vr_tree* mt = const_cast<vr_tree*>(t);
     std::lock_guard<std::mutex> host_lock(mt->host_mu);   // one host-path sweep per tree at a time
     vr_tree::HostPath& R = mt->host;
@@ -1195,7 +641,6 @@ int vr_tree_eval(const vr_tree* t, const float* xyz_dev, const float* dir_dev, i
 int vr_draw_probe(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, const float probe_xyz[3],
                   int disp_size, const vr_rect* tile, uint8_t* rgba8_dev, float* rgba32f_dev,
                   unsigned long long rgba8_surf, void* stream_) {
-    if (n_views < 0) return fail(VR_EINVAL, "n_views < 0");
     if (!probe_xyz) return fail(VR_EINVAL, "null probe position");
     if (rgba8_surf) {
         if (n_views != 1 || tile || rgba8_dev || rgba32f_dev)
@@ -1203,11 +648,9 @@ int vr_draw_probe(const vr_tree* t, const vr_camera* cams, int n_views, const vr
     } else if (!rgba8_dev && !rgba32f_dev) {
         return fail(VR_EINVAL, "no output to draw into");
     }
-    if (n_views == 0) return VR_OK;
     vr_rect r;
-    int rc = check_common(t, cams, opt, tile, r);
-    if (rc) return rc;
-    if ((rc = same_size(cams, n_views))) return rc;
+    const int rc = check_batch(t, cams, n_views, opt, tile, r);
+    if (rc || n_views == 0) return rc;
     if (coef0_only(t))
         return fail(VR_EUNSUPPORTED, "probe unavailable for basis_dim %d (only coefficient 0 is resident)", t->dev.basis_dim);
     if (disp_size <= 0) return VR_OK;   // the reference's candidate pixels then all lie outside the disc
@@ -1404,7 +847,6 @@ int vr_tree_wireframe(const vr_tree* t, int max_depth, float* vert_dev, int64_t 
     if (e != cudaSuccess) return cuda_fail(e, "wireframe");
     return VR_OK;
 }
-
 
 // estimate_normals (mesh.cpp:63-97) on a device vertex buffer (kernels: vr_normals.cu).
 int vr_mesh_estimate_normals(float* vert_dev, int64_t n_verts, const uint32_t* faces_dev, int64_t n_faces,

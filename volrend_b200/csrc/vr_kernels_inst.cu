@@ -49,7 +49,7 @@ int resident_ctas(K kernel, size_t smem, int num_sms) {
 void set_work(LaunchDev& P, const LaunchCfg& cfg, bool blocks = true) {
     P.tiles_x = (P.w + kTW - 1) / kTW;
     P.tiles_y = (P.h + kTH - 1) / kTH;
-    P.work_counter = cfg.queue;
+    P.work_counter = cfg.work_counter;
     // Batches have the queue hand out blocks of 64 tiles, the warps of an SM sharing a block (vr_march.cuh next_item).
     // Up to 16 basis functions: 4x4 tiles of 4 consecutive views, view innermost, so that the colour records
     // neighbouring poses share are read from the SM's L1 instead of from L2 (DESIGN.md 4: modelled record L1 hit rate
@@ -80,7 +80,6 @@ template <typename K>
 cudaError_t launch_persistent_grid(K kernel, size_t smem, LaunchDev& P, const LaunchCfg& cfg, bool blocks = true) {
     set_work(P, cfg, blocks);
     int grid = resident_ctas(kernel, smem, cfg.num_sms);
-    if (cfg.max_ctas > 0 && grid > cfg.max_ctas) grid = cfg.max_ctas;
     const int need = (P.n_tiles + (kBlock / 32) - 1) / (kBlock / 32);
     if (grid > need) grid = need;
     if (grid < 1) grid = 1;
@@ -111,40 +110,24 @@ cudaError_t launch_queue(LaunchDev& P, const LaunchCfg& cfg) {
 
 }  // namespace
 
-// variant 0: the default for this basis size
-template <int KBD>
-bool variant_supported(int variant) {
-    if (variant == 0 || variant == kVariantInline) return true;
-    return variant == kVariantQueue && KBD >= 4;
-}
-
 template <int KBD>
 cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg) {
-    int variant = cfg.variant;
-    if (!variant_supported<KBD>(variant)) return cudaErrorInvalidValue;
-    // Default (DESIGN.md 4).  The queue pays ~30 instructions per march iteration (ballots, ring bookkeeping) for a 3x denser colour block: a
-    // loss in batches, where other warps hide the inline block's latency, a win on single frames, where the long-ray
-    // tail of the frame is what is waited for.  With 25 basis functions its per-ray basis values (112 B) push the CTA's
-    // shared memory over the 8-CTA budget.  Both kernels produce identical bits.
-    if (variant == 0) variant = (P.n_views == 1 && KBD >= 4 && KBD <= 16) ? kVariantQueue : kVariantInline;
-    const bool queue = variant == kVariantQueue;
     if (P.opts) {   // options per view (vr_render_batch_opts): no surface output
         if (cfg.surface) return cudaErrorInvalidValue;
         if (cfg.count)
-            return queue ? launch_queue<KBD, true, kOutViewOpts>(P, cfg) : launch_persistent<KBD, true, kOutViewOpts>(P, cfg);
-        return queue ? launch_queue<KBD, false, kOutViewOpts>(P, cfg) : launch_persistent<KBD, false, kOutViewOpts>(P, cfg);
+            return cfg.queue ? launch_queue<KBD, true, kOutViewOpts>(P, cfg) : launch_persistent<KBD, true, kOutViewOpts>(P, cfg);
+        return cfg.queue ? launch_queue<KBD, false, kOutViewOpts>(P, cfg) : launch_persistent<KBD, false, kOutViewOpts>(P, cfg);
     }
     if (cfg.surface) {  // drop-in launch_renderer path writing the caller's cudaArray
-        return queue ? launch_queue<KBD, false, kOutSurface>(P, cfg) : launch_persistent<KBD, false, kOutSurface>(P, cfg);
+        return cfg.queue ? launch_queue<KBD, false, kOutSurface>(P, cfg) : launch_persistent<KBD, false, kOutSurface>(P, cfg);
     }
     if (cfg.count) {  // instrumented builds
-        return queue ? launch_queue<KBD, true, kOutLinear>(P, cfg) : launch_persistent<KBD, true, kOutLinear>(P, cfg);
+        return cfg.queue ? launch_queue<KBD, true, kOutLinear>(P, cfg) : launch_persistent<KBD, true, kOutLinear>(P, cfg);
     }
-    return queue ? launch_queue<KBD, false, kOutLinear>(P, cfg) : launch_persistent<KBD, false, kOutLinear>(P, cfg);
+    return cfg.queue ? launch_queue<KBD, false, kOutLinear>(P, cfg) : launch_persistent<KBD, false, kOutLinear>(P, cfg);
 }
 
 template cudaError_t launch_march<VR_KBD>(LaunchDev&, const LaunchCfg&);
-template bool variant_supported<VR_KBD>(int);
 
 #if VR_KBD == 1
 // KBD 0: no basis set-up and no parked ray constants (the weights march reads no record)
