@@ -120,20 +120,19 @@ __device__ __forceinline__ unsigned short leaf_half(const LeafSrc& S, long long 
     return S.colors[((size_t)q * 65536 + S.qmap[(size_t)q * S.n_slots + slot]) * 3 + k];
 }
 
-// nodes[i]: absolute child id, or leaf bit | sigma.  Also validates child links.
+// Node word of a link outside [1, capacity): neither a node id (< 2^28) nor a leaf word.  Only an error when the
+// depth sweep reaches it -- the reference never follows the links of unreachable nodes.
+constexpr uint32_t kBadLink = 0x7fffffffu;
+
+// nodes[i]: absolute child id, leaf bit | sigma, or kBadLink.
 __global__ void relayout_nodes_kernel(const int32_t* __restrict__ child, LeafSrc S, uint32_t* __restrict__ nodes,
-                                      long long capacity, int* __restrict__ bad) {
+                                      long long capacity) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= S.n_slots) return;
     const int32_t rel = child[i];
     if (rel != 0) {
         const long long tgt = (i >> 3) + rel;
-        if (tgt <= 0 || tgt >= capacity) {
-            atomicExch(bad, 1);
-            nodes[i] = kLeafBit;
-        } else {
-            nodes[i] = (uint32_t)tgt;
-        }
+        nodes[i] = (tgt <= 0 || tgt >= capacity) ? kBadLink : (uint32_t)tgt;
     } else {
         nodes[i] = kLeafBit | (uint32_t)leaf_sigma(S, i);
     }
@@ -141,7 +140,7 @@ __global__ void relayout_nodes_kernel(const int32_t* __restrict__ child, LeafSrc
 
 // depth[n] of every node by level-synchronous relaxation from the root.  A node that is reached
 // twice (two parents, or a cycle) makes the input a DAG, not a tree: rejected, because the table
-// builder and the ancestor stacks assume one depth per node.
+// builder and the ancestor stacks assume one depth per node.  So is a reached link outside [1, capacity).
 __global__ void node_depth_kernel(const uint32_t* __restrict__ nodes, int* __restrict__ depth, long long capacity,
                                   int level, int* __restrict__ flags) {
     const long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -149,7 +148,9 @@ __global__ void node_depth_kernel(const uint32_t* __restrict__ nodes, int* __res
 #pragma unroll
     for (int s = 0; s < 8; ++s) {
         const uint32_t w = nodes[n * 8 + s];
-        if (!(w & kLeafBit)) {
+        if (w == kBadLink) {
+            atomicExch(flags, 1);
+        } else if (!(w & kLeafBit)) {
             if (atomicCAS(&depth[w], -1, level + 1) != -1) atomicExch(flags + 2, 1);
             flags[1] = 1;
         }
@@ -356,7 +357,7 @@ static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, 
         VR_CUDA(cudaMalloc(&t->extra, nf * sizeof(float)));
         VR_CUDA(cudaMemcpy(t->extra, d->extra, nf * sizeof(float), cudaMemcpyHostToDevice));
     }
-    relayout_nodes_kernel<<<(unsigned)((n_slots + TB - 1) / TB), TB>>>(raw_child, S, t->nodes, d->capacity, flags);
+    relayout_nodes_kernel<<<(unsigned)((n_slots + TB - 1) / TB), TB>>>(raw_child, S, t->nodes, d->capacity);
     VR_CUDA(cudaGetLastError());
     release(raw_child);
 
