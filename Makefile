@@ -2,6 +2,8 @@
 #   make lib      volrend_b200/libvolrend_b200.so   the product: C-ABI + sm_90a kernels
 #   make oracle   oracle/liboracle.so               CPU restatement (test infrastructure), and
 #                 oracle/libprobe_oracle.so         the same with the probe disc
+#                 oracle/libweights_oracle.so       ... with the leaf-weights pass
+#                 oracle/libgrads_oracle.so         ... with the leaf-gradient pass
 #                 oracle/libsurface_harness.so      cudaArray + surface objects for the surface render path's tests
 #   make ref      oracle/_ref/*                     the unmodified reference (+ its gen_wireframe, probe and mesh harnesses), built from
 #                                                   $(VOLREND_REF) (only when it exists)
@@ -74,12 +76,14 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp volrend_b200/csrc/vr_frames.h incl
 $(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
-oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libsurface_harness.so
+oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/libsurface_harness.so
 oracle/liboracle.so: oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 oracle/libprobe_oracle.so: oracle/probe_oracle.c oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 oracle/libweights_oracle.so: oracle/weights_oracle.c oracle/march_oracle.c oracle/march_oracle.h
+	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
+oracle/libgrads_oracle.so: oracle/grads_oracle.c oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 oracle/libsurface_harness.so: oracle/surface_harness.cu
 	$(NVCC) $(ARCH) -O2 -std=c++17 -Xcompiler -fPIC -shared -o $@ $<
@@ -97,4 +101,4 @@ shim:
 	 else echo "reference tree $(VOLREND_REF) not present: shim needs the reference headers"; fi
 
 clean:
-	rm -rf build $(LIB) oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libsurface_harness.so oracle/_ref
+	rm -rf build $(LIB) oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/libsurface_harness.so oracle/_ref

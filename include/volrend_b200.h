@@ -176,6 +176,27 @@ int vr_tree_leaf_weights(const vr_tree* tree, const vr_camera* cams, int n_views
                          const vr_rect* tile, float* weight_dev, float* alpha_dev, vr_counters* counters_dev,
                          void* stream);
 
+/* Gradient of the float output of vr_render_batch w.r.t. every leaf's data row (fitting leaf values to images).
+ * dpix_dev: tile-sized float4 per view (dL/d{r,g,b,alpha} of the rgba32f output); grad_dev: capacity*8*data_dim floats
+ * on the tree's device, slot-major like N3Tree::data_ (slot = node*8 + octant), ACCUMULATED into (caller initialises,
+ * e.g. to 0).  rgba32f_dev: NULL, or receives the float output of the forward replay (bit-identical to
+ * vr_render_batch's).  The samples are vr_render_batch's; every shaded sample adds its terms with one atomicAdd each
+ * (formulas in DESIGN.md 18), so the sums depend on the order of the atomics and are not bit-reproducible from run to
+ * run.  Columns the device does not keep (coefficients k >= 1 of a basis size without its own kernel, columns between
+ * the colour coefficients and sigma) get nothing, nor do internal and free slots.  render_depth is VR_EINVAL, a tree
+ * created without VR_TREE_SLOT_MAP VR_EUNSUPPORTED; otherwise validated as vr_render_batch.  Asynchronous on stream. */
+int vr_tree_leaf_grads(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
+                       const vr_rect* tile, const float* dpix_dev, float* grad_dev, float* rgba32f_dev, void* stream);
+
+/* Replace the leaf values of a tree created with VR_TREE_SLOT_MAP: data_dev is fp16 [capacity*8*data_dim] on the
+ * tree's device, laid out as vr_tree_desc::data.  Every table entry whose wslot names a leaf gets that slot's colour
+ * record and the sigma bits of its leaf word rewritten (under table parity 1 several entries name one slot: all are
+ * written); structure, parity, tables and sizes (vr_tree_get_info) do not change, and renders, vr_tree_query,
+ * vr_tree_eval and vr_probe_lumisphere read the new values.  VR_EUNSUPPORTED without the slot map, VR_EINVAL for NULL
+ * data or data on another device.  Asynchronous on stream: ordering against launches on other streams that read the
+ * tree is the caller's job. */
+int vr_tree_update_data(vr_tree* tree, const uint16_t* data_dev, void* stream);
+
 /* launch_renderer(offscreen=false): rgba8_dev is read (existing colour) and overwritten;
  * depth_dev holds the per-pixel ray-distance limit (world units), both tile-sized. */
 int vr_render_composite(const vr_tree* tree, const vr_camera* cam, const vr_options* opt,

@@ -59,6 +59,19 @@ int vrb::need_device(const vr_tree* t) {
     return VR_OK;
 }
 
+int vrb::buffer_check(const vr_tree* t, const void* p, const char* what) {
+    if (!p) return VR_OK;
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(VR_EINVAL, "%s is not a CUDA allocation", what);
+    }
+    if (a.type == cudaMemoryTypeUnregistered) return fail(VR_EINVAL, "%s is not device memory", what);
+    if (a.type == cudaMemoryTypeDevice && a.device != t->device)
+        return fail(VR_EINVAL, "%s lives on device %d, the tree on device %d", what, a.device, t->device);
+    return VR_OK;
+}
+
 namespace {
 // f(std::integral_constant<int, K>{}) for the kernel bases K the march kernels are built for (kbd_built); `otherwise`
 // for any other kbd.
@@ -157,12 +170,15 @@ int stream_res(vr_tree* t, cudaStream_t stream, StreamRes*& out) {
     return VR_OK;
 }
 
-// One launch of P.n_views views, on the kernel march_kernel() picks.  weights: the weights pass (one kernel for every
-// basis size, whatever the variant setting).
-int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStream_t stream, bool weights = false) {
+// What a march launch computes: the render, the weights pass (one kernel for every basis size) or the gradient pass
+// (one kernel per basis size); the two passes ignore the variant setting.
+enum class Pass { kRender, kWeights, kGrads };
+
+// One launch of P.n_views views, on the kernel march_kernel() picks.
+int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStream_t stream, Pass pass = Pass::kRender) {
     const int variant = vr_get_variant();
     const MarchKernel kernel = march_kernel(t->dev.kbd, variant, P.n_views);
-    if (!weights && kernel == MarchKernel::kNotBuilt)
+    if (pass == Pass::kRender && kernel == MarchKernel::kNotBuilt)
         return fail(VR_EUNSUPPORTED, "kernel variant %d is not available for kernel basis %d", variant, t->dev.kbd);
     LaunchCfg cfg;
     cfg.queue = kernel == MarchKernel::kQueue;
@@ -175,8 +191,8 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
         cfg.work_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(sr->queues) + (size_t)(sr->next_queue++ % kQueueSlots) * kQueueSlotBytes);
     }
     // march_kernel above has rejected every kbd without kernels
-    const cudaError_t e = weights ? launch_weights(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
-        return launch_march<decltype(k)::value>(P, cfg);
+    const cudaError_t e = pass == Pass::kWeights ? launch_weights(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
+        return pass == Pass::kGrads ? launch_grads<decltype(k)::value>(P, cfg) : launch_march<decltype(k)::value>(P, cfg);
     });
     if (e != cudaSuccess) return fail(VR_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     g_launches += 1;
@@ -252,9 +268,9 @@ int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_
 // hold h rows of w pixels per view); this adds the tree, the cameras and the options, and launches the views in chunks
 // that fit the camera ring and the 31-bit tile index, the output pointers advanced to each chunk's first view.
 // opt_stride as in vr_frames.h; a chunk of one view is an ordinary single-view launch with that view's options.
-// weights: the weights pass, P.alpha advanced like the outputs.
+// pass: the weights or gradient pass, P.alpha and P.dpix advanced like the outputs.
 int march(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
-          const LaunchDev& P, bool surface, cudaStream_t stream, bool weights = false) {
+          const LaunchDev& P, bool surface, cudaStream_t stream, Pass pass = Pass::kRender) {
     const long long tb = tile_bound(vr_rect{P.x0, P.y0, P.w, P.h});
     const int max_views = tb * kCamRing > 0x7fffffffLL ? (int)(0x7fffffffLL / tb) : kCamRing;
     const size_t px = (size_t)P.w * P.h;
@@ -269,8 +285,9 @@ int march(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options
         C.rgbaf = skip(P.rgbaf, px * v0);
         C.depth_in = skip(P.depth_in, px * v0);
         C.alpha = skip(P.alpha, px * v0);
+        C.dpix = skip(P.dpix, px * v0);
         if (int rc = stage_cams(t, cams + v0, nv, stream, C, opt_stride ? o : nullptr)) return rc;
-        return dispatch(t, C, P.counters != nullptr, surface, stream, weights);
+        return dispatch(t, C, P.counters != nullptr, surface, stream, pass);
     });
 }
 
@@ -357,7 +374,28 @@ int vr_tree_leaf_weights(const vr_tree* t, const vr_camera* cams, int n_views, c
     P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
     P.counters = counters_dev;
     P.wslot = t->wslot; P.weights = weight_dev; P.alpha = alpha_dev;
-    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, true);
+    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, Pass::kWeights);
+}
+
+int vr_tree_leaf_grads(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
+                       const vr_rect* tile, const float* dpix_dev, float* grad_dev, float* rgba32f_dev, void* stream) {
+    if (n_views > 0 && (!dpix_dev || !grad_dev)) return fail(VR_EINVAL, "null dpix or gradient buffer");
+    vr_rect r;
+    int rc = check_batch(t, cams, n_views, opt, tile, r);
+    if (rc || n_views == 0) return rc;
+    if (opt->render_depth) return fail(VR_EINVAL, "leaf gradients are of the colour output: render_depth is not supported");
+    if (!t->wslot)
+        return fail(VR_EUNSUPPORTED, "leaf gradients need the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if ((rc = buffer_check(t, dpix_dev, "dpix_dev")) || (rc = buffer_check(t, grad_dev, "grad_dev")) ||
+        (rc = buffer_check(t, rgba32f_dev, "rgba32f_dev")))
+        return rc;
+    if (r.w == 0 || r.h == 0) return VR_OK;
+    LaunchDev P{};
+    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
+    P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
+    P.wslot = t->wslot;
+    P.dpix = reinterpret_cast<const float4*>(dpix_dev); P.grad = grad_dev; P.grad_dim = t->data_dim;
+    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, Pass::kGrads);
 }
 
 int vr_render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
@@ -574,21 +612,6 @@ static int query_check(const vr_tree* t, const float* xyz, int64_t n, bool* full
     return VR_OK;
 }
 
-// The kernel dereferences `p`: it must be memory the tree's device can address (not pageable host memory, not
-// another device's allocation).
-static int query_buffer_check(const vr_tree* t, const void* p, const char* what) {
-    if (!p) return VR_OK;
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(VR_EINVAL, "%s is not a CUDA allocation", what);
-    }
-    if (a.type == cudaMemoryTypeUnregistered) return fail(VR_EINVAL, "%s is not device memory", what);
-    if (a.type == cudaMemoryTypeDevice && a.device != t->device)
-        return fail(VR_EINVAL, "%s lives on device %d, the tree on device %d", what, a.device, t->device);
-    return VR_OK;
-}
-
 // query_single_from_root (n3tree_query.hpp:13-48) for n world points (kernel: vr_query.cu).
 int vr_tree_query(const vr_tree* t, const float* xyz_dev, int64_t n, uint16_t* data_dev, float* cube_dev,
                   float* local_dev, void* stream_) {
@@ -601,8 +624,8 @@ int vr_tree_query(const vr_tree* t, const float* xyz_dev, int64_t n, uint16_t* d
                     coef0_only(t) ? "only coefficient 0" : "the colour coefficients and sigma only");
     if (n == 0 || (!data_dev && !cube_dev && !local_dev)) return VR_OK;
     int bc;
-    if ((bc = query_buffer_check(t, xyz_dev, "xyz_dev")) || (bc = query_buffer_check(t, data_dev, "data_dev")) ||
-        (bc = query_buffer_check(t, cube_dev, "cube_dev")) || (bc = query_buffer_check(t, local_dev, "local_dev")))
+    if ((bc = buffer_check(t, xyz_dev, "xyz_dev")) || (bc = buffer_check(t, data_dev, "data_dev")) ||
+        (bc = buffer_check(t, cube_dev, "cube_dev")) || (bc = buffer_check(t, local_dev, "local_dev")))
         return bc;
     QueryLaunch Q{};
     Q.tree = t->dev;
@@ -624,8 +647,8 @@ int vr_tree_eval(const vr_tree* t, const float* xyz_dev, const float* dir_dev, i
         return fail(VR_EUNSUPPORTED, "eval unavailable for basis_dim %d (only coefficient 0 is resident)", t->dev.basis_dim);
     if (n == 0 || (!rgb_dev && !sigma_dev)) return VR_OK;
     int bc;
-    if ((bc = query_buffer_check(t, xyz_dev, "xyz_dev")) || (rgb_dev && (bc = query_buffer_check(t, dir_dev, "dir_dev"))) ||
-        (bc = query_buffer_check(t, rgb_dev, "rgb_dev")) || (bc = query_buffer_check(t, sigma_dev, "sigma_dev")))
+    if ((bc = buffer_check(t, xyz_dev, "xyz_dev")) || (rgb_dev && (bc = buffer_check(t, dir_dev, "dir_dev"))) ||
+        (bc = buffer_check(t, rgb_dev, "rgb_dev")) || (bc = buffer_check(t, sigma_dev, "sigma_dev")))
         return bc;
     QueryLaunch Q{};
     Q.tree = t->dev;

@@ -45,11 +45,22 @@ cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg);
 // reads no colour record, so one kernel serves every basis size; it is built in the VR_KBD=1 object.
 cudaError_t launch_weights(LaunchDev& P, const LaunchCfg& cfg);
 
+// The gradient pass of vr_tree_leaf_grads: the inline-shading kernel's kOutGrads instantiation for kernel basis KBD
+// (it reads the colour records), built in each basis size's object.
+template <int KBD>
+cudaError_t launch_grads(LaunchDev& P, const LaunchCfg& cfg);
+
 extern template cudaError_t launch_march<-1>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<1>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<4>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<9>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<16>(LaunchDev&, const LaunchCfg&);
 extern template cudaError_t launch_march<25>(LaunchDev&, const LaunchCfg&);
+extern template cudaError_t launch_grads<-1>(LaunchDev&, const LaunchCfg&);
+extern template cudaError_t launch_grads<1>(LaunchDev&, const LaunchCfg&);
+extern template cudaError_t launch_grads<4>(LaunchDev&, const LaunchCfg&);
+extern template cudaError_t launch_grads<9>(LaunchDev&, const LaunchCfg&);
+extern template cudaError_t launch_grads<16>(LaunchDev&, const LaunchCfg&);
+extern template cudaError_t launch_grads<25>(LaunchDev&, const LaunchCfg&);
 
 }  // namespace vrb

@@ -9,7 +9,8 @@
 //                      and the bench
 // Both also come as kOutViewOpts instantiations (plain and counting), which read each view's options from
 // LaunchDev::opts: batches with options per view.  The VR_KBD=1 object also holds the weights pass
-// (march_persistent_kernel<0, *, kOutWeights>, vr_tree_leaf_weights), one kernel for every basis size.
+// (march_persistent_kernel<0, *, kOutWeights>, vr_tree_leaf_weights), one kernel for every basis size, and every object
+// the gradient pass of its basis size (march_persistent_kernel<VR_KBD, false, kOutGrads>, vr_tree_leaf_grads).
 #include <mutex>
 
 #include "vr_kernels.h"
@@ -128,6 +129,14 @@ cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg) {
 }
 
 template cudaError_t launch_march<VR_KBD>(LaunchDev&, const LaunchCfg&);
+
+// no parked ray constants: the gradient march keeps its ray in registers
+template <int KBD>
+cudaError_t launch_grads(LaunchDev& P, const LaunchCfg& cfg) {
+    return launch_persistent_grid(march_persistent_kernel<KBD, false, kOutGrads>, march_smem_bytes(P.tree.max_depth), P, cfg);
+}
+
+template cudaError_t launch_grads<VR_KBD>(LaunchDev&, const LaunchCfg&);
 
 #if VR_KBD == 1
 // KBD 0: no basis set-up and no parked ray constants (the weights march reads no record)

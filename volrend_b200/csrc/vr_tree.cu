@@ -214,8 +214,9 @@ __global__ void build_wide_kernel(const uint32_t* __restrict__ nodes, const int*
 
 // wrecs[entry]: padded colour record of the entry's leaf, straight from the source arrays
 // (16-byte chunks; 8-byte records as one chunk).  Entries that are not leaves stay zero.
+// wide != nullptr (vr_tree_update_data): also the sigma bits (low 16) of every leaf entry's word, from the same source.
 __global__ void build_wrecs_kernel(const uint32_t* __restrict__ wslot, LeafSrc S, unsigned char* __restrict__ wrecs,
-                                   long long n_entries, int rec_bytes) {
+                                   long long n_entries, int rec_bytes, uint32_t* __restrict__ wide = nullptr) {
     const int chunks = rec_bytes >= 16 ? rec_bytes / 16 : 1;
     const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long e = gid / chunks;
@@ -223,6 +224,7 @@ __global__ void build_wrecs_kernel(const uint32_t* __restrict__ wslot, LeafSrc S
     if (e >= n_entries) return;
     const uint32_t slot = wslot[e];
     const bool leaf = slot != 0xffffffffu;
+    if (wide && leaf && c == 0) wide[e] = (wide[e] & 0xffff0000u) | leaf_sigma(S, slot);
     if (rec_bytes == 8) {
         ushort4 v = make_ushort4(0, 0, 0, 0);
         if (leaf) { v.x = leaf_half(S, slot, 0); v.y = leaf_half(S, slot, 1); v.z = leaf_half(S, slot, 2); }
@@ -473,6 +475,26 @@ int vr_tree_create_quantized_ex(const vr_tree_quant_desc* q, uint32_t flags, vr_
     return tree_create_impl(&q->base, q, flags, out);
 }
 int vr_tree_create_quantized(const vr_tree_quant_desc* q, vr_tree** out) { return vr_tree_create_quantized_ex(q, 0, out); }
+
+int vr_tree_update_data(vr_tree* t, const uint16_t* data_dev, void* stream) {
+    if (!t) return fail(VR_EINVAL, "null tree");
+    if (int rc = need_device(t)) return rc;
+    if (!t->wslot)
+        return fail(VR_EUNSUPPORTED, "updating leaf data needs the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if (!data_dev) return fail(VR_EINVAL, "null data");
+    if (int rc = buffer_check(t, data_dev, "data_dev")) return rc;
+    LeafSrc S{};
+    S.data = data_dev;
+    S.n_slots = t->info.capacity * 8; S.data_dim = t->data_dim; S.basis_dim = t->dev.basis_dim; S.kbd = t->dev.kbd;
+    const long long n_entries = t->dev.wide_entries;
+    const int rec_bytes = t->dev.rec_bytes, TB = 256;
+    const long long rwork = n_entries * (rec_bytes >= 16 ? rec_bytes / 16 : 1);
+    build_wrecs_kernel<<<(unsigned)((rwork + TB - 1) / TB), TB, 0, (cudaStream_t)stream>>>(t->wslot, S, t->wrecs,
+                                                                                            n_entries, rec_bytes, t->wide);
+    VR_CUDA(cudaGetLastError());
+    g_launches += 1;
+    return VR_OK;
+}
 
 int vr_tree_get_info(const vr_tree* t, vr_tree_info* info) {
     if (!t || !info) return fail(VR_EINVAL, "null argument");

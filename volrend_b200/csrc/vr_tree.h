@@ -20,6 +20,10 @@ extern std::atomic<unsigned long long> g_launches;
 // launches pay no more); without one, some device must exist.
 int need_device(const vr_tree* t);
 
+// A buffer a kernel dereferences: NULL, or memory the tree's device can address (not pageable host memory, not another
+// device's allocation); `what` names it in the error.
+int buffer_check(const vr_tree* t, const void* p, const char* what);
+
 // A failed CUDA call: VR_ENOMEM for an allocation, else VR_ECUDA, with the message "<what>: <CUDA's text><where>".
 // The runtime's last error is cleared, so that a later launch check does not report this failure again.
 inline int cuda_fail(cudaError_t e, const char* what, const char* where = "") {
@@ -56,7 +60,7 @@ struct vr_tree {
     unsigned char* wrecs = nullptr;
     float* extra = nullptr;
     // upload scratch (slot-indexed node words, table entry -> slot), freed once the tables are built; with
-    // VR_TREE_SLOT_MAP the table entry -> slot map stays (vr_tree_leaf_weights)
+    // VR_TREE_SLOT_MAP the table entry -> slot map stays (vr_tree_leaf_weights, vr_tree_leaf_grads, vr_tree_update_data)
     uint32_t* nodes = nullptr;
     uint32_t* wslot = nullptr;
     long long n_tables = 0;

@@ -114,6 +114,11 @@ struct LaunchDev {
     const uint32_t* wslot;
     float* weights;
     float* alpha;
+    // leaf gradients (vr_tree_leaf_grads), read only by the kOutGrads instantiations, which also use wslot and rgbaf:
+    // dL/d(pixel) per pixel, the caller's gradient rows of grad_dim (= data_dim) floats per slot.  Last, as above.
+    const float4* dpix;
+    float* grad;
+    int32_t grad_dim;
 };
 
 }  // namespace vrb

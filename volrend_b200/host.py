@@ -278,6 +278,29 @@ class N3Tree:
         d.ndc_width, d.ndc_height, d.ndc_focal = self.ndc_width, self.ndc_height, self.ndc_focal
         return d, data
 
+    def update_data(self, data, stream=None) -> None:
+        """Replaces the leaf values on the device (vr_tree_update_data): ``data`` is a CUDA tensor on the tree's device,
+        fp16 or fp32 (rounded with ``.half()``), shaped like ``data_``.  The structure does not change.  The host copy
+        of the data, and the compressed arrays of a quantised file, are dropped (``clear_cpu_memory``), so this object
+        never describes two different trees.  Asynchronous on ``stream``.  The tree must be loaded with
+        ``load_cuda(slot_map=True)``."""
+        import torch
+        if not self.is_cuda_loaded():
+            raise RuntimeError("N3Tree is not loaded on the device")
+        if not self._slot_map:
+            raise RuntimeError("update_data needs the slot map: load the tree with load_cuda(slot_map=True)")
+        shape = (self.capacity, self.N, self.N, self.N, self.data_dim)
+        dev = torch.device("cuda", self._device)
+        if (not isinstance(data, torch.Tensor) or data.dtype not in (torch.float16, torch.float32)
+                or data.device != dev or tuple(data.shape) != shape):
+            raise ValueError(f"data must be a float16 or float32 tensor of shape {shape} on {dev}")
+        h = data.half().contiguous()
+        check(lib().vr_tree_update_data(self._handle, h.data_ptr(), _stream_ptr(stream)))
+        if stream is not None and isinstance(stream, torch.cuda.Stream) and h is not data:
+            h.record_stream(stream)     # the temporary is read by the kernel on `stream`
+        self.clear_cpu_memory()
+        self.quant_ = None
+
     def free_cuda(self) -> None:
         if self._handle is not None:
             lib().vr_tree_destroy(self._handle)
@@ -672,6 +695,48 @@ def leaf_weights(tree: N3Tree, cams, options: RenderOptions, out=None, alpha=Non
     check(lib().vr_tree_leaf_weights(tree._handle, arr, len(cams), C.byref(o), _rect(tile), out.data_ptr(),
                                      alpha.data_ptr() if alpha is not None else None,
                                      counters.data_ptr() if counters is not None else None, _stream_ptr(stream)))
+    return out
+
+
+def leaf_grads(tree: N3Tree, cams, options: RenderOptions, dpix, out=None, float_out=None, stream=None, *, tile=None):
+    """Gradient of a loss on the float render of the views ``cams`` w.r.t. every leaf's data row (vr_tree_leaf_grads):
+    ``dpix`` is dL/d(r, g, b, alpha) of each pixel, a contiguous float32 CUDA tensor ``[V, H, W, 4]`` (tile-sized), and
+    the result a float32 tensor ``[capacity, 2, 2, 2, data_dim]`` laid out like ``data_``.  ``out`` (that shape or as
+    many elements, on the tree's device) accumulates over calls; without it a new tensor starts at 0.  ``float_out``:
+    optional float32 ``[V, H, W, 4]`` that receives the render the gradient is of (``render_batch``'s ``float_out``,
+    bit for bit).  ``options`` is one RenderOptions; ``render_depth`` is refused.  Asynchronous on ``stream``; the sums
+    are atomic, so they vary in the last bits from run to run.  The tree must be loaded with
+    ``load_cuda(slot_map=True)``."""
+    import torch
+    if not tree.is_cuda_loaded():
+        raise RuntimeError("N3Tree is not loaded on the device")
+    if not tree._slot_map:
+        raise RuntimeError("leaf_grads needs the slot map: load the tree with load_cuda(slot_map=True)")
+    if isinstance(cams, Camera):
+        cams = [cams]
+    if not isinstance(options, RenderOptions):
+        raise TypeError("leaf_grads takes one RenderOptions for every view")
+    dev = torch.device("cuda", tree._device)
+    n = tree.capacity * tree.N ** 3 * tree.data_dim
+    if out is None:
+        out = torch.zeros((tree.capacity, tree.N, tree.N, tree.N, tree.data_dim), dtype=torch.float32, device=dev)
+    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
+          or not out.is_contiguous() or out.numel() != n):
+        raise ValueError(f"out must be a contiguous float32 tensor of {n} elements on {dev}")
+    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if cams else (0, 0)
+    npx = len(cams) * w * h * 4
+    for name, t in (("dpix", dpix), ("float_out", float_out)):
+        if t is None and name == "float_out":
+            continue
+        if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous()
+                or t.numel() != npx):
+            raise ValueError(f"{name} must be a contiguous float32 tensor of {len(cams)} x {h} x {w} x 4 elements "
+                             f"on {dev}")
+    arr = _cams_array(cams)
+    o = options._as_c()
+    check(lib().vr_tree_leaf_grads(tree._handle, arr, len(cams), C.byref(o), _rect(tile), dpix.data_ptr(),
+                                   out.data_ptr(), float_out.data_ptr() if float_out is not None else None,
+                                   _stream_ptr(stream)))
     return out
 
 

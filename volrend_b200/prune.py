@@ -150,12 +150,9 @@ def read_intrinsics(path: str):
     return float(vals[0]), float(vals[5])
 
 
-def _parser() -> argparse.ArgumentParser:
-    ap = argparse.ArgumentParser(prog="python -m volrend_b200.prune",
-                                 description="Prune a PlenOctree npz by ray weight: leaves whose maximum compositing "
-                                             "weight over the given views is below --thresh are dropped.")
-    ap.add_argument("input", help="npz file storing octree data (uncompressed)")
-    ap.add_argument("output", help="where to write the pruned npz")
+def add_view_arguments(ap: argparse.ArgumentParser) -> None:
+    """The camera, pose and march options of the tools that run views over a tree (prune, finetune):
+    volrend_headless's pose files, -i, -r and image size, and the step and thresholds."""
     ap.add_argument("poses", nargs="+", help="camera-to-world pose .txt files (row-major 4x4, one or more per file)")
     ap.add_argument("-i", "--intrin", default="", help="intrinsics matrix 4x4; if set, overrides the fx/fy")
     ap.add_argument("-r", "--reverse_yz", action="store_true", help="use OpenCV camera space convention instead of NeRF")
@@ -166,6 +163,48 @@ def _parser() -> argparse.ArgumentParser:
     ap.add_argument("--step_size", type=float, default=1e-4, help="ray march step size")
     ap.add_argument("--sigma_thresh", type=float, default=1e-2, help="sigma threshold of a shaded sample")
     ap.add_argument("--stop_thresh", type=float, default=1e-2, help="transmittance below which a ray stops")
+
+
+def view_setup(ap: argparse.ArgumentParser, args):
+    """Checks add_view_arguments' values (ap.error on a bad one) -> (row-major 4x4 poses, fx, fy)."""
+    if args.width < 1 or args.height < 1:
+        ap.error(f"image size {args.width}x{args.height} must be positive")
+    for p in args.poses + ([args.intrin] if args.intrin else []):
+        if not os.path.exists(p):
+            ap.error(f"'{p}' does not exist")
+    fx = 1111.11 if args.fx < 0 else args.fx
+    fy = fx if args.fy < 0 else args.fy
+    if args.intrin:
+        fx, fy = read_intrinsics(args.intrin)
+    poses = [m for p in args.poses for m in read_poses(p)]
+    if not poses:
+        ap.error("no camera poses in the pose files")
+    if args.reverse_yz:
+        poses = [m @ np.diag([1, -1, -1, 1]).astype(np.float32) for m in poses]
+    return poses, fx, fy
+
+
+def load_tree_arrays(d: dict, path: str):
+    """An N3Tree of the npz dict ``d`` read from ``path``, on the device with the slot map; NDC trees (a
+    ``<tree>_poses_bounds.npy`` beside the file) as ``N3Tree.open`` loads them."""
+    from .host import N3Tree
+    tree = N3Tree()
+    tree.load_npz(d)
+    pb = path[:-4] + "_poses_bounds.npy"
+    if path.endswith(".npz") and os.path.exists(pb):
+        tree.use_ndc = True
+        tree._unpack_llff_poses_bounds(np.load(pb))
+    tree.load_cuda(slot_map=True)
+    return tree
+
+
+def _parser() -> argparse.ArgumentParser:
+    ap = argparse.ArgumentParser(prog="python -m volrend_b200.prune",
+                                 description="Prune a PlenOctree npz by ray weight: leaves whose maximum compositing "
+                                             "weight over the given views is below --thresh are dropped.")
+    ap.add_argument("input", help="npz file storing octree data (uncompressed)")
+    ap.add_argument("output", help="where to write the pruned npz")
+    add_view_arguments(ap)
     ap.add_argument("--thresh", type=float, default=1e-3, help="leaves with a maximum weight below this are dropped")
     ap.add_argument("--no-collapse", dest="collapse", action="store_false",
                     help="keep internal nodes whose children are all dropped")
@@ -184,31 +223,16 @@ def main(argv=None) -> int:
         ap.error(f"--batch {args.batch} < 1")
     if os.path.abspath(args.input) == os.path.abspath(args.output):
         ap.error("the output would overwrite the input")
-    for p in [args.input] + args.poses + ([args.intrin] if args.intrin else []):
-        if not os.path.exists(p):
-            ap.error(f"'{p}' does not exist")
-    fx = 1111.11 if args.fx < 0 else args.fx
-    fy = fx if args.fy < 0 else args.fy
-    if args.intrin:
-        fx, fy = read_intrinsics(args.intrin)
-    poses = [m for p in args.poses for m in read_poses(p)]
-    if not poses:
-        ap.error("no camera poses in the pose files")
-    if args.reverse_yz:
-        poses = [m @ np.diag([1, -1, -1, 1]).astype(np.float32) for m in poses]
+    if not os.path.exists(args.input):
+        ap.error(f"'{args.input}' does not exist")
+    poses, fx, fy = view_setup(ap, args)
     with np.load(args.input) as z:
         d = {k: z[k] for k in z.files}
     if "quant_map" in d or "quant_colors" in d:
         ap.error(f"{args.input} is already compressed: prune the uncompressed tree first, then compress")
 
-    from .host import Camera, N3Tree, RenderOptions, leaf_weights
-    tree = N3Tree()
-    tree.load_npz(d)
-    pb = args.input[:-4] + "_poses_bounds.npy"
-    if args.input.endswith(".npz") and os.path.exists(pb):   # NDC trees, as N3Tree.open
-        tree.use_ndc = True
-        tree._unpack_llff_poses_bounds(np.load(pb))
-    tree.load_cuda(slot_map=True)
+    from .host import Camera, RenderOptions, leaf_weights
+    tree = load_tree_arrays(d, args.input)
     opt = RenderOptions(step_size=args.step_size, sigma_thresh=args.sigma_thresh, stop_thresh=args.stop_thresh)
     cams = []
     for m in poses:
