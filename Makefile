@@ -4,6 +4,7 @@
 #                 oracle/libprobe_oracle.so         the same with the probe disc
 #                 oracle/libweights_oracle.so       ... with the leaf-weights pass
 #                 oracle/libgrads_oracle.so         ... with the leaf-gradient pass
+#                 oracle/liberror_oracle.so         ... with the leaf-error pass
 #                 oracle/libsurface_harness.so      cudaArray + surface objects for the surface render path's tests
 #   make ref      oracle/_ref/*                     the unmodified reference (+ its gen_wireframe, probe and mesh harnesses), built from
 #                                                   $(VOLREND_REF) (only when it exists)
@@ -76,7 +77,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp volrend_b200/csrc/vr_frames.h incl
 $(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
-oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/libsurface_harness.so
+oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/liberror_oracle.so oracle/libsurface_harness.so
 oracle/liboracle.so: oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 oracle/libprobe_oracle.so: oracle/probe_oracle.c oracle/march_oracle.c oracle/march_oracle.h
@@ -84,6 +85,8 @@ oracle/libprobe_oracle.so: oracle/probe_oracle.c oracle/march_oracle.c oracle/ma
 oracle/libweights_oracle.so: oracle/weights_oracle.c oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 oracle/libgrads_oracle.so: oracle/grads_oracle.c oracle/march_oracle.c oracle/march_oracle.h
+	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
+oracle/liberror_oracle.so: oracle/error_oracle.c oracle/march_oracle.c oracle/march_oracle.h
 	$(CC) -O2 -ffp-contract=off -fno-fast-math -fPIC -shared -pthread -o $@ $< -lm
 oracle/libsurface_harness.so: oracle/surface_harness.cu
 	$(NVCC) $(ARCH) -O2 -std=c++17 -Xcompiler -fPIC -shared -o $@ $<
@@ -101,4 +104,4 @@ shim:
 	 else echo "reference tree $(VOLREND_REF) not present: shim needs the reference headers"; fi
 
 clean:
-	rm -rf build $(LIB) oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/libsurface_harness.so oracle/_ref
+	rm -rf build $(LIB) oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/liberror_oracle.so oracle/libsurface_harness.so oracle/_ref

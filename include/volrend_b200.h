@@ -176,6 +176,20 @@ int vr_tree_leaf_weights(const vr_tree* tree, const vr_camera* cams, int n_views
                          const vr_rect* tile, float* weight_dev, float* alpha_dev, vr_counters* counters_dev,
                          void* stream);
 
+/* Per-leaf sum of compositing weight x pixel error over n_views views (choosing the leaves to split when refining a
+ * fitted tree).  Every shaded sample (sigma > sigma_thresh) of every pixel of `tile` (NULL = full frame) of every view
+ * adds  w_i * err[view][pixel]  to score_dev[slot] (slot = node*8 + octant in the source arrays), w_i = T_i (1 - att_i)
+ * computed by exactly the operations of vr_tree_leaf_weights' weights.  err_dev: tile-sized floats per view;
+ * score_dev: capacity*8 floats, ACCUMULATED into (caller initialises, e.g. to 0).  Every ray is marched whatever its
+ * err (an err of 0 adds zeros), so counters_dev accumulates exactly the counters of vr_tree_leaf_weights.  One
+ * atomicAdd per shaded sample: the sums depend on the order of the atomics and are not bit-reproducible from run to
+ * run.  Of `opt`, the same fields act as in vr_tree_leaf_weights.  VR_EUNSUPPORTED for a tree created without
+ * VR_TREE_SLOT_MAP; VR_EINVAL for NULL err_dev / score_dev or buffers that are not device memory of the tree's
+ * device; otherwise validated as vr_render_batch.  Asynchronous on stream. */
+int vr_tree_leaf_error(const vr_tree* tree, const vr_camera* cams, int n_views, const vr_options* opt,
+                       const vr_rect* tile, const float* err_dev, float* score_dev, vr_counters* counters_dev,
+                       void* stream);
+
 /* Gradient of the float output of vr_render_batch w.r.t. every leaf's data row (fitting leaf values to images).
  * dpix_dev: tile-sized float4 per view (dL/d{r,g,b,alpha} of the rgba32f output); grad_dev: capacity*8*data_dim floats
  * on the tree's device, slot-major like N3Tree::data_ (slot = node*8 + octant), ACCUMULATED into (caller initialises,

@@ -73,6 +73,8 @@ SYMBOLS = {
     "vr_tree_create_quantized_ex": (C.c_int, [C.POINTER(vr_tree_quant_desc), C.c_uint32, C.POINTER(C.c_void_p)]),
     "vr_tree_leaf_weights": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
                                        C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vr_tree_leaf_error": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
+                                     C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_tree_leaf_grads": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
                                      C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_tree_update_data": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -170,9 +170,9 @@ int stream_res(vr_tree* t, cudaStream_t stream, StreamRes*& out) {
     return VR_OK;
 }
 
-// What a march launch computes: the render, the weights pass (one kernel for every basis size) or the gradient pass
-// (one kernel per basis size); the two passes ignore the variant setting.
-enum class Pass { kRender, kWeights, kGrads };
+// What a march launch computes: the render, the weights or error pass (one kernel for every basis size) or the
+// gradient pass (one kernel per basis size); the passes ignore the variant setting.
+enum class Pass { kRender, kWeights, kGrads, kError };
 
 // One launch of P.n_views views, on the kernel march_kernel() picks.
 int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStream_t stream, Pass pass = Pass::kRender) {
@@ -191,7 +191,7 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
         cfg.work_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(sr->queues) + (size_t)(sr->next_queue++ % kQueueSlots) * kQueueSlotBytes);
     }
     // march_kernel above has rejected every kbd without kernels
-    const cudaError_t e = pass == Pass::kWeights ? launch_weights(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
+    const cudaError_t e = pass == Pass::kWeights ? launch_weights(P, cfg) : pass == Pass::kError ? launch_error(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
         return pass == Pass::kGrads ? launch_grads<decltype(k)::value>(P, cfg) : launch_march<decltype(k)::value>(P, cfg);
     });
     if (e != cudaSuccess) return fail(VR_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
@@ -268,7 +268,7 @@ int stage_cams(const vr_tree* t, const vr_camera* cams, int n_views, cudaStream_
 // hold h rows of w pixels per view); this adds the tree, the cameras and the options, and launches the views in chunks
 // that fit the camera ring and the 31-bit tile index, the output pointers advanced to each chunk's first view.
 // opt_stride as in vr_frames.h; a chunk of one view is an ordinary single-view launch with that view's options.
-// pass: the weights or gradient pass, P.alpha and P.dpix advanced like the outputs.
+// pass: the weights, gradient or error pass, P.alpha, P.dpix and P.err advanced like the outputs.
 int march(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, int opt_stride,
           const LaunchDev& P, bool surface, cudaStream_t stream, Pass pass = Pass::kRender) {
     const long long tb = tile_bound(vr_rect{P.x0, P.y0, P.w, P.h});
@@ -286,6 +286,7 @@ int march(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options
         C.depth_in = skip(P.depth_in, px * v0);
         C.alpha = skip(P.alpha, px * v0);
         C.dpix = skip(P.dpix, px * v0);
+        C.err = skip(P.err, px * v0);
         if (int rc = stage_cams(t, cams + v0, nv, stream, C, opt_stride ? o : nullptr)) return rc;
         return dispatch(t, C, P.counters != nullptr, surface, stream, pass);
     });
@@ -375,6 +376,24 @@ int vr_tree_leaf_weights(const vr_tree* t, const vr_camera* cams, int n_views, c
     P.counters = counters_dev;
     P.wslot = t->wslot; P.weights = weight_dev; P.alpha = alpha_dev;
     return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, Pass::kWeights);
+}
+
+int vr_tree_leaf_error(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
+                       const vr_rect* tile, const float* err_dev, float* score_dev, vr_counters* counters_dev,
+                       void* stream) {
+    if (n_views > 0 && (!err_dev || !score_dev)) return fail(VR_EINVAL, "null err or score buffer");
+    vr_rect r;
+    int rc = check_batch(t, cams, n_views, opt, tile, r);
+    if (rc || n_views == 0) return rc;
+    if (!t->wslot)
+        return fail(VR_EUNSUPPORTED, "leaf error needs the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if ((rc = buffer_check(t, err_dev, "err_dev")) || (rc = buffer_check(t, score_dev, "score_dev"))) return rc;
+    if (r.w == 0 || r.h == 0) return VR_OK;
+    LaunchDev P{};
+    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
+    P.counters = counters_dev;
+    P.wslot = t->wslot; P.err = err_dev; P.score = score_dev;
+    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, Pass::kError);
 }
 
 int vr_tree_leaf_grads(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,

@@ -45,6 +45,10 @@ cudaError_t launch_march(LaunchDev& P, const LaunchCfg& cfg);
 // reads no colour record, so one kernel serves every basis size; it is built in the VR_KBD=1 object.
 cudaError_t launch_weights(LaunchDev& P, const LaunchCfg& cfg);
 
+// The error pass of vr_tree_leaf_error: the kOutError instantiation, the weights pass's march summing weight * err;
+// like the weights pass, one kernel for every basis size in the VR_KBD=1 object.
+cudaError_t launch_error(LaunchDev& P, const LaunchCfg& cfg);
+
 // The gradient pass of vr_tree_leaf_grads: the inline-shading kernel's kOutGrads instantiation for kernel basis KBD
 // (it reads the colour records), built in each basis size's object.
 template <int KBD>

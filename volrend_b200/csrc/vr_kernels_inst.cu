@@ -9,8 +9,9 @@
 //                      and the bench
 // Both also come as kOutViewOpts instantiations (plain and counting), which read each view's options from
 // LaunchDev::opts: batches with options per view.  The VR_KBD=1 object also holds the weights pass
-// (march_persistent_kernel<0, *, kOutWeights>, vr_tree_leaf_weights), one kernel for every basis size, and every object
-// the gradient pass of its basis size (march_persistent_kernel<VR_KBD, false, kOutGrads>, vr_tree_leaf_grads).
+// (march_persistent_kernel<0, *, kOutWeights>, vr_tree_leaf_weights) and the error pass (<0, *, kOutError>,
+// vr_tree_leaf_error), one kernel each for every basis size, and every object the gradient pass of its basis size
+// (march_persistent_kernel<VR_KBD, false, kOutGrads>, vr_tree_leaf_grads).
 #include <mutex>
 
 #include "vr_kernels.h"
@@ -144,6 +145,12 @@ cudaError_t launch_weights(LaunchDev& P, const LaunchCfg& cfg) {
     const size_t smem = march_smem_bytes(P.tree.max_depth);
     if (cfg.count) return launch_persistent_grid(march_persistent_kernel<0, true, kOutWeights>, smem, P, cfg);
     return launch_persistent_grid(march_persistent_kernel<0, false, kOutWeights>, smem, P, cfg);
+}
+
+cudaError_t launch_error(LaunchDev& P, const LaunchCfg& cfg) {
+    const size_t smem = march_smem_bytes(P.tree.max_depth);
+    if (cfg.count) return launch_persistent_grid(march_persistent_kernel<0, true, kOutError>, smem, P, cfg);
+    return launch_persistent_grid(march_persistent_kernel<0, false, kOutError>, smem, P, cfg);
 }
 #endif
 

@@ -119,6 +119,10 @@ struct LaunchDev {
     const float4* dpix;
     float* grad;
     int32_t grad_dim;
+    // leaf error (vr_tree_leaf_error), read only by the kOutError instantiations, which also use wslot: the per-pixel
+    // error and the caller's per-slot sums.  Last, as above.
+    const float* err;
+    float* score;
 };
 
 }  // namespace vrb

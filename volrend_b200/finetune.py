@@ -4,13 +4,15 @@
                                     [-i intrinsics.txt] [-r] [--width 800] [--height 800] [--fx F] [--fy F]
                                     [--step_size S] [--sigma_thresh S] [--stop_thresh S] [--background B]
                                     [--steps 100] [--lr 1e-2] [--batch 4] [--seed 0] [--holdout K]
+                                    [--refine-every K] [--refine-fraction 0.1] [--max-depth 23]
 
 The fit uses the march's own samples: the renders are ``render_batch``'s float output and the gradients come from the
 same samples on the GPU (``vr_tree_leaf_grads``, see :func:`volrend_b200.leaf_grads`; formulas in DESIGN.md section
 18), so a lower loss is a better picture in the viewer.  An fp32 master copy of the data lives on the device; each step
 renders a batch of views, takes the MSE on RGB against the targets, back-propagates it to the leaves, takes one Adam
-step on the master and writes it, rounded to fp16, into the device tree (``N3Tree.update_data``).  The structure never
-changes.  Columns the device does not keep (coefficients of a basis size without its own kernel beyond the first, and
+step on the master and writes it, rounded to fp16, into the device tree (``N3Tree.update_data``).  The structure
+changes only with ``--refine-every K``: every K steps the leaves that carry the most residual error are split
+(coarse-to-fine, :mod:`volrend_b200.refine`, DESIGN.md section 19).  Columns the device does not keep (coefficients of a basis size without its own kernel beyond the first, and
 SG / ASG lobes) get no gradient and keep their values.
 
 Targets are one PNG per pose or one ``.npy`` of shape [V, H, W, 3 | 4], uint8 or float in [0, 1].  RGBA targets are
@@ -44,18 +46,29 @@ def _target_rgb(img, background: float, device):
     return t
 
 
-def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int, seed: int, on_step=None):
+def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int, seed: int, on_step=None,
+             refine_every: int = 0, refine_fraction: float = 0.1, max_depth: int = 23, on_refine=None):
     """Fits the leaf data of ``tree`` (an ``N3Tree`` loaded with ``load_cuda(slot_map=True)`` that still holds its host
     data) to ``targets``: a sequence of one image per camera in ``cams`` ([H, W, 3 | 4], uint8 or float, indexed
     lazily, so it may read files on demand).  Each of ``steps`` steps takes the next ``batch`` views of a shuffle seeded
     with ``seed`` (reshuffled after every pass), renders them with ``options``, back-propagates the MSE on RGB and takes
     one ``torch.optim.Adam`` step (learning rate ``lr``) on an fp32 master copy of the data, which is then written into
     the device tree.  ``on_step(step, loss)`` is called after every step.  Returns ``(master, losses)``: the fp32 data
-    ``[capacity, 2, 2, 2, data_dim]`` on the device and the loss of every step.  The tree's host data is dropped."""
+    ``[capacity, 2, 2, 2, data_dim]`` on the device and the loss of every step.  The tree's host data is dropped.
+
+    Coarse-to-fine: with ``refine_every = K > 0``, before every step ``s = K, 2K, ... < steps`` the leaves are scored
+    over all of ``cams`` (:func:`volrend_b200.refine.leaf_scores`, batches of ``batch`` views) and split by
+    :func:`volrend_b200.refine_plan` (``refine_fraction``, ``max_depth``); the master and both Adam moments are
+    gathered by its ``src`` (a new slot starts with its parent's value and moments, the step count carries on), the
+    device tree is re-created with the slot map from ``master.half()`` and ``on_refine(step, n_split, nodes_before,
+    nodes_after)`` is called.  ``tree`` (``child_``, ``capacity``) then describes the refined tree."""
     import torch
     from .host import leaf_grads, render_batch
+    from .refine import leaf_scores, refine_plan
     if steps < 0 or batch < 1:
         raise ValueError(f"steps {steps} must be >= 0 and batch {batch} >= 1")
+    if refine_every < 0:
+        raise ValueError(f"refine_every {refine_every} must be >= 0")
     if len(targets) != len(cams):
         raise ValueError(f"{len(targets)} targets for {len(cams)} views")
     if not cams:
@@ -74,6 +87,20 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
     grad = torch.zeros_like(master)
     losses = []
     for step in range(steps):
+        if refine_every > 0 and step > 0 and step % refine_every == 0:
+            scores = leaf_scores(tree, cams, targets, options, batch).cpu().numpy().reshape(-1)
+            child, src = refine_plan(tree.child_, scores, refine_fraction, max_depth)
+            n0, n1 = tree.capacity, child.shape[0]
+            if n1 > n0:
+                master, opt = _gather_fit(master, opt, lr, torch.from_numpy(src).to(dev))
+                grad = torch.zeros_like(master)
+                tree.child_, tree.capacity = np.ascontiguousarray(child), n1
+                tree.quant_ = None
+                tree.data_ = master.detach().half().cpu().numpy()
+                tree.load_cuda(slot_map=True)
+                tree.clear_cpu_memory()
+            if on_refine is not None:
+                on_refine(step, n1 - n0, n0, n1)
         if pos + nb > len(cams):
             order, pos = gen.permutation(len(cams)), 0
         views = order[pos:pos + nb]
@@ -97,10 +124,27 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
     return master.detach(), losses
 
 
-def finetune_npz(z, data) -> dict:
+def _gather_fit(master, opt, lr, src):
+    """The fp32 master copy and a new Adam over it with every per-slot tensor (value, both moments) gathered by the
+    source slot index ``src`` (``refine_plan``); the step count carries over."""
+    import torch
+    dd = master.shape[-1]
+    take = lambda x: x.detach().reshape(-1, dd)[src].reshape(-1, 2, 2, 2, dd)
+    new = take(master).requires_grad_(True)
+    opt2 = torch.optim.Adam([new], lr=lr)
+    st = opt.state.get(master)
+    if st:
+        opt2.state[new] = {"step": st["step"].clone(), "exp_avg": take(st["exp_avg"]),
+                           "exp_avg_sq": take(st["exp_avg_sq"])}
+    return new, opt2
+
+
+def finetune_npz(z, data, *, child=None) -> dict:
     """The tree dict ``z`` (``N3Tree`` npz keys) with ``data`` (the fitted leaf values, [capacity, 2, 2, 2, data_dim],
     numpy or torch) written in the source's dtype; keys as :func:`volrend_b200.prune_npz` (the training-time keys
-    ``compress_npz`` drops are dropped, every other key passes through).  Compressed input (``quant_map``) is refused."""
+    ``compress_npz`` drops are dropped, every other key passes through).  ``child``: the structure of a fit with
+    refinement (``N3Tree.child_`` after :func:`finetune`), written with ``data`` of its capacity; without it the
+    structure is ``z``'s.  Compressed input (``quant_map``) is refused."""
     keys = list(z.files if hasattr(z, "files") else z)
     if "quant_map" in keys or "quant_colors" in keys:
         raise ValueError("the tree is compressed (quant_map): fine-tune the uncompressed tree, then prune and compress")
@@ -109,10 +153,13 @@ def finetune_npz(z, data) -> dict:
             raise ValueError(f"the tree has no '{k}' array")
     src = np.asarray(z["data"])
     d = data.detach().cpu().numpy() if hasattr(data, "detach") else np.asarray(data)
-    if d.shape != src.shape:
-        raise ValueError(f"data has shape {d.shape}, the tree's {src.shape}")
+    shape = src.shape if child is None else np.asarray(child).shape + src.shape[-1:]
+    if d.shape != shape:
+        raise ValueError(f"data has shape {d.shape}, the tree's {shape}")
     out = {k: z[k] for k in keys if k != "data" and k not in DROPPED_KEYS}
     out["data"] = d.astype(src.dtype)
+    if child is not None:
+        out["child"] = np.asarray(child, np.int32)
     return out
 
 
@@ -176,6 +223,12 @@ def _parser() -> argparse.ArgumentParser:
     ap.add_argument("--batch", type=int, default=4, help="views per step")
     ap.add_argument("--seed", type=int, default=0, help="seed of the view shuffle")
     ap.add_argument("--holdout", type=int, default=0, help="the last K poses are held out: PSNR before and after")
+    ap.add_argument("--refine-every", type=int, default=0,
+                    help="every K steps, split the leaves with the most residual error (0: never; the structure stays)")
+    ap.add_argument("--refine-fraction", type=float, default=0.1,
+                    help="share of the candidate leaves split at each refinement, in [0, 1]")
+    ap.add_argument("--max-depth", type=int, default=23,
+                    help="leaves at this depth (root's slots = 1) or deeper are not split (at most 23)")
     return ap
 
 
@@ -202,6 +255,12 @@ def main(argv=None) -> int:
         ap.error(f"--batch {args.batch} < 1")
     if not (args.lr > 0) or math.isinf(args.lr):
         ap.error(f"--lr {args.lr} must be a positive number")
+    if args.refine_every < 0:
+        ap.error(f"--refine-every {args.refine_every} < 0")
+    if not (0.0 <= args.refine_fraction <= 1.0):
+        ap.error(f"--refine-fraction {args.refine_fraction} must be in [0, 1]")
+    if args.max_depth < 1:
+        ap.error(f"--max-depth {args.max_depth} < 1")
     if os.path.abspath(args.input) == os.path.abspath(args.output):
         ap.error("the output would overwrite the input")
     for p in [args.input] + args.targets:
@@ -234,10 +293,13 @@ def main(argv=None) -> int:
         print(f"held-out PSNR before: {_psnr(tree, cams, targets, held, opt):.3f} dB")
     master, _ = finetune(tree, cams[:n_train], targets[:n_train], opt,
                          steps=args.steps, lr=args.lr, batch=args.batch, seed=args.seed,
-                         on_step=lambda s, l: print(f"step {s}: loss {l:.6g}"))
+                         on_step=lambda s, l: print(f"step {s}: loss {l:.6g}"),
+                         refine_every=args.refine_every, refine_fraction=args.refine_fraction,
+                         max_depth=args.max_depth,
+                         on_refine=lambda s, n, a, b: print(f"refine before step {s}: split {n}, nodes {a} -> {b}"))
     if held:
         print(f"held-out PSNR after: {_psnr(tree, cams, targets, held, opt):.3f} dB")
-    out = finetune_npz(d, master)
+    out = finetune_npz(d, master, child=tree.child_ if args.refine_every > 0 else None)
     tree.free_cuda()
     _write_npz(args.output, out)
     return 0

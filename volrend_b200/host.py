@@ -698,6 +698,43 @@ def leaf_weights(tree: N3Tree, cams, options: RenderOptions, out=None, alpha=Non
     return out
 
 
+def leaf_error(tree: N3Tree, cams, options: RenderOptions, err, out=None, counters=None, stream=None, *, tile=None):
+    """Per-leaf residual error over the views ``cams`` (vr_tree_leaf_error): a CUDA float32 tensor
+    ``[capacity, 2, 2, 2]`` (slot = node * 8 + octant) to which every shaded sample of every pixel has added its
+    compositing weight T * (1 - att) times the pixel's ``err``, a contiguous float32 CUDA tensor ``[V, H, W]``
+    (tile-sized; e.g. the squared colour error of a render).  ``out`` (same shape or ``capacity * 8`` elements, float32,
+    on the tree's device) accumulates over calls; without it a new tensor starts at 0.  ``options`` is one
+    RenderOptions (the fields that act in :func:`leaf_weights` act here).  ``counters``: optional int64[5] device
+    tensor, accumulated.  Asynchronous on ``stream``; the sums are atomic, so they vary in the last bits from run to
+    run.  The tree must be loaded with ``load_cuda(slot_map=True)``."""
+    import torch
+    if not tree.is_cuda_loaded():
+        raise RuntimeError("N3Tree is not loaded on the device")
+    if not tree._slot_map:
+        raise RuntimeError("leaf_error needs the slot map: load the tree with load_cuda(slot_map=True)")
+    if isinstance(cams, Camera):
+        cams = [cams]
+    if not isinstance(options, RenderOptions):
+        raise TypeError("leaf_error takes one RenderOptions for every view")
+    dev = torch.device("cuda", tree._device)
+    n_slots = tree.capacity * tree.N ** 3
+    if out is None:
+        out = torch.zeros((tree.capacity, tree.N, tree.N, tree.N), dtype=torch.float32, device=dev)
+    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
+          or not out.is_contiguous() or out.numel() != n_slots):
+        raise ValueError(f"out must be a contiguous float32 tensor of {n_slots} elements on {dev}")
+    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if cams else (0, 0)
+    if (not isinstance(err, torch.Tensor) or err.dtype != torch.float32 or err.device != dev
+            or not err.is_contiguous() or err.numel() != len(cams) * w * h):
+        raise ValueError(f"err must be a contiguous float32 tensor of {len(cams)} x {h} x {w} elements on {dev}")
+    arr = _cams_array(cams)
+    o = options._as_c()
+    check(lib().vr_tree_leaf_error(tree._handle, arr, len(cams), C.byref(o), _rect(tile), err.data_ptr(),
+                                   out.data_ptr(), counters.data_ptr() if counters is not None else None,
+                                   _stream_ptr(stream)))
+    return out
+
+
 def leaf_grads(tree: N3Tree, cams, options: RenderOptions, dpix, out=None, float_out=None, stream=None, *, tile=None):
     """Gradient of a loss on the float render of the views ``cams`` w.r.t. every leaf's data row (vr_tree_leaf_grads):
     ``dpix`` is dL/d(r, g, b, alpha) of each pixel, a contiguous float32 CUDA tensor ``[V, H, W, 4]`` (tile-sized), and
