@@ -211,6 +211,30 @@ int vr_tree_leaf_grads(const vr_tree* tree, const vr_camera* cams, int n_views, 
  * tree is the caller's job. */
 int vr_tree_update_data(vr_tree* tree, const uint16_t* data_dev, void* stream);
 
+/* Forward neighbours of every leaf (the total-variation prior of vr_tree_leaf_tv).  A reachable leaf slot at depth d
+ * (root's slots: 1) with integer cell i in [0, 2^d)^3 of the tree's unit cube has, along axis a, the neighbour
+ * n_a = the leaf whose cell holds the point (i + e_a) 2^-d, found by a descent from the root: the leaf that covers a
+ * coarser or equal region across the +a face, the leaf at the min-corner octant of a finer one; none when
+ * i_a + 1 = 2^d.  nbr_dev: capacity*8*3 int32 on the tree's device, nbr[slot*3 + a] = n_a or -1; internal, free and
+ * unreachable slots get -1 in all three.  Cell counts are taken on the first call for a tree (shared with
+ * vr_tree_wireframe; that call synchronises stream).  VR_EUNSUPPORTED for a tree created without VR_TREE_SLOT_MAP,
+ * VR_EINVAL for a NULL buffer or one that is not device memory of the tree's device.  Asynchronous on stream. */
+int vr_tree_leaf_neighbors(const vr_tree* tree, int32_t* nbr_dev, void* stream);
+
+/* Total variation between neighbouring leaves (DESIGN.md 20), on the fp32 rows data_dev [capacity*8*data_dim]:
+ *   E = sum_G (lambda_G / N_leaf) sum_{leaf s} sum_{c in G} sqrt(1e-8 + sum_{a: n_a(s) exists} (v[n_a, c] - v[s, c])^2)
+ * over the groups G = sigma (column data_dim - 1) and colour (the coefficient columns vr_tree_leaf_grads writes);
+ * N_leaf is the number of reachable leaf slots and n_a comes from nbr_dev, vr_tree_leaf_neighbors' table of this
+ * tree.  dE/dv is ACCUMULATED into grad_dev (capacity*8*data_dim floats, e.g. vr_tree_leaf_grads' buffer) and E added
+ * to *energy_dev (one double on the device; NULL: not computed).  Other columns and non-leaf slots get nothing; a
+ * group whose weight is 0 is skipped, and with both weights 0 nothing is launched.  The gradient terms are float
+ * atomicAdds: the sums depend on the order of the atomics and are not bit-reproducible from run to run.  VR_EINVAL for
+ * a negative or non-finite weight, NULL nbr / data / grad or buffers that are not device memory of the tree's device;
+ * VR_EUNSUPPORTED without the slot map.  Asynchronous on stream (the first call for a tree may synchronise it, as in
+ * vr_tree_leaf_neighbors). */
+int vr_tree_leaf_tv(const vr_tree* tree, const int32_t* nbr_dev, const float* data_dev, float lambda_sigma,
+                    float lambda_color, float* grad_dev, double* energy_dev, void* stream);
+
 /* launch_renderer(offscreen=false): rgba8_dev is read (existing colour) and overwritten;
  * depth_dev holds the per-pixel ray-distance limit (world units), both tile-sized. */
 int vr_render_composite(const vr_tree* tree, const vr_camera* cam, const vr_options* opt,

@@ -78,6 +78,9 @@ SYMBOLS = {
     "vr_tree_leaf_grads": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.c_int, C.POINTER(vr_options),
                                      C.POINTER(vr_rect), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vr_tree_update_data": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vr_tree_leaf_neighbors": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vr_tree_leaf_tv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
     "vr_tree_destroy": (None, [C.c_void_p]),
     "vr_tree_get_info": (C.c_int, [C.c_void_p, C.POINTER(vr_tree_info)]),
     "vr_render": (C.c_int, [C.c_void_p, C.POINTER(vr_camera), C.POINTER(vr_options), C.POINTER(vr_rect),

@@ -23,6 +23,7 @@
 #include "vr_query.h"
 #include "vr_raster.h"
 #include "vr_tree.h"
+#include "vr_tv.h"
 #include "vr_wire.h"
 
 using namespace vrb;
@@ -859,34 +860,103 @@ int vr_draw_meshes_batch(const vr_camera* cams, int n_views, const vr_mesh_desc*
     return VR_OK;
 }
 
+}  // extern "C"
+
+namespace {
+// The tree as the wireframe walk reads it.
+WireTree wire_tree(const vr_tree* t) {
+    WireTree w{};
+    w.wide = t->wide; w.n_tables = t->n_tables; w.wide_p = t->dev.wide_p; w.max_level = t->dev.max_depth;
+    for (int i = 0; i < 3; ++i) { w.offset[i] = t->dev.offset[i]; w.scale[i] = t->dev.scale[i]; }
+    return w;
+}
+
+// The tree's cells per level (t->wire_levels), counted on the first call (which synchronises `stream`).
+int ensure_wire_levels(const vr_tree* t, const WireTree& w, cudaStream_t stream) {
+    vr_tree* mt = const_cast<vr_tree*>(t);
+    std::lock_guard<std::mutex> lk(mt->wire_mu);
+    if (!mt->wire_ready) {
+        int launches = 0;
+        const cudaError_t e = wire_levels(w, mt->wire_levels, stream, &launches);
+        g_launches += launches;
+        if (e != cudaSuccess) return cuda_fail(e, "wireframe cell count");
+        mt->wire_ready = true;
+    }
+    return VR_OK;
+}
+}  // namespace
+
+extern "C" {
+
 // N3Tree::gen_wireframe (n3tree.cpp:365-434) from the device tables (kernels: vr_wire.cu).
 int vr_tree_wireframe(const vr_tree* t, int max_depth, float* vert_dev, int64_t max_verts, int64_t* n_verts_out,
                       void* stream_) {
     if (!t || !n_verts_out) return fail(VR_EINVAL, "null argument");
     if (int rc = need_device(t)) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
-    vr_tree* mt = const_cast<vr_tree*>(t);
-    WireTree w{};
-    w.wide = t->wide; w.n_tables = t->n_tables; w.wide_p = t->dev.wide_p; w.max_level = t->dev.max_depth;
-    for (int i = 0; i < 3; ++i) { w.offset[i] = t->dev.offset[i]; w.scale[i] = t->dev.scale[i]; }
-    int launches = 0;
-    {
-        std::lock_guard<std::mutex> lk(mt->wire_mu);
-        if (!mt->wire_ready) {
-            const cudaError_t e = wire_levels(w, mt->wire_levels, stream, &launches);
-            g_launches += launches;
-            if (e != cudaSuccess) return cuda_fail(e, "wireframe cell count");
-            mt->wire_ready = true;
-        }
-    }
+    const WireTree w = wire_tree(t);
+    if (int rc = ensure_wire_levels(t, w, stream)) return rc;
     const long long n = 24 * wire_cells(w, t->wire_levels, max_depth);
     *n_verts_out = n;
     if (!vert_dev) return VR_OK;
     if (max_verts < n) return fail(VR_EINVAL, "the wireframe at max_depth %d has %lld vertices, the buffer holds %lld", max_depth, n, (long long)max_verts);
-    launches = 0;
+    int launches = 0;
     const cudaError_t e = wire_fill(w, t->wire_levels, max_depth, vert_dev, stream, &launches);
     g_launches += launches;
     if (e != cudaSuccess) return cuda_fail(e, "wireframe");
+    return VR_OK;
+}
+
+// Forward neighbours of every leaf slot (kernels: vr_tv.cu, on the wireframe's walk).
+int vr_tree_leaf_neighbors(const vr_tree* t, int32_t* nbr_dev, void* stream_) {
+    if (!t) return fail(VR_EINVAL, "null tree");
+    int rc = need_device(t);
+    if (rc) return rc;
+    if (!t->wslot)
+        return fail(VR_EUNSUPPORTED, "leaf neighbours need the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if (!nbr_dev) return fail(VR_EINVAL, "null neighbour buffer");
+    if ((rc = buffer_check(t, nbr_dev, "nbr_dev"))) return rc;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const WireTree w = wire_tree(t);
+    if ((rc = ensure_wire_levels(t, w, stream))) return rc;
+    int launches = 0;
+    const cudaError_t e = tv_neighbors(w, t->wire_levels, t->dev, t->wslot, t->info.capacity * 8, nbr_dev, stream,
+                                       &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) return cuda_fail(e, "leaf neighbours");
+    return VR_OK;
+}
+
+// Total variation between neighbouring leaves, its gradient added to grad_dev (kernels: vr_tv.cu).
+int vr_tree_leaf_tv(const vr_tree* t, const int32_t* nbr_dev, const float* data_dev, float lambda_sigma,
+                    float lambda_color, float* grad_dev, double* energy_dev, void* stream_) {
+    if (!t) return fail(VR_EINVAL, "null tree");
+    int rc = need_device(t);
+    if (rc) return rc;
+    if (!(lambda_sigma >= 0.f) || !(lambda_color >= 0.f) || std::isinf(lambda_sigma) || std::isinf(lambda_color))
+        return fail(VR_EINVAL, "TV weights must be finite and >= 0 (sigma %g, colour %g)", lambda_sigma, lambda_color);
+    if (!t->wslot)
+        return fail(VR_EUNSUPPORTED, "leaf TV needs the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if (!nbr_dev || !data_dev || !grad_dev) return fail(VR_EINVAL, "null neighbour, data or gradient buffer");
+    if ((rc = buffer_check(t, nbr_dev, "nbr_dev")) || (rc = buffer_check(t, data_dev, "data_dev")) ||
+        (rc = buffer_check(t, grad_dev, "grad_dev")) || (rc = buffer_check(t, energy_dev, "energy_dev")))
+        return rc;
+    if (lambda_sigma == 0.f && lambda_color == 0.f) return VR_OK;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const WireTree w = wire_tree(t);
+    if ((rc = ensure_wire_levels(t, w, stream))) return rc;
+    long long n_leaf = 0;
+    for (int l = 0; l < kWireLevels; ++l) n_leaf += t->wire_levels.leaf[l];
+    // the columns of vr_tree_leaf_grads: RGBA channels 0..2, or coefficient k < kbd of channel c at c * basis_dim + k
+    TvColumns cols;
+    cols.data_dim = t->data_dim;
+    cols.n_coef = t->dev.kbd > 0 ? t->dev.kbd : 1;
+    cols.coef_stride = t->dev.kbd > 0 ? t->dev.basis_dim : 1;
+    int launches = 0;
+    const cudaError_t e = tv_pass(data_dev, nbr_dev, t->info.capacity * 8, cols, (double)lambda_sigma / n_leaf,
+                                  (double)lambda_color / n_leaf, grad_dev, energy_dev, stream, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) return cuda_fail(e, "leaf TV");
     return VR_OK;
 }
 

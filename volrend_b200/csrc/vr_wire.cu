@@ -2,9 +2,8 @@
 // generated on the device from the wide tables, bit for bit.  See DESIGN.md section 9.
 //
 // The reference walks the host tree depth first and pushes 24 vertices per emitted cell.  Here the cells are
-// generated level by level (one thread per table entry), keyed by their Morton code, sorted (which restores the
-// depth-first pre-order), and expanded to vertices.
-#include <cooperative_groups.h>
+// generated level by level (one thread per table entry, vr_wire_walk.cuh), keyed by their Morton code, sorted (which
+// restores the depth-first pre-order), and expanded to vertices.
 #include <cub/device/device_radix_sort.cuh>
 #include <cuda/std/tuple>
 
@@ -15,21 +14,14 @@
 
 #include "vr_types.h"
 #include "vr_wire.h"
-
-namespace cg = cooperative_groups;
+#include "vr_wire_walk.cuh"
 
 namespace vrb {
 namespace {
 
-constexpr int kTB = 256;
 constexpr int kWriteCells = 32;        // cells per CTA of the vertex writer
 constexpr int kCellFloats = 24 * 9;    // 12 segments = 24 vertices of position, colour, normal
 constexpr int kKey64Levels = 21;       // 3 bits per level
-
-// A node the expansion visits: its table id and its integer corner on the grid of its own depth.
-struct WireNode {
-    uint32_t table, x, y, z;
-};
 
 // Cell order.  The reference visits octants x-major, then y, then z, and descends before moving on, so its output
 // order is the order of the cells' Morton codes (x the most significant bit of each level) once every corner is
@@ -86,78 +78,22 @@ __device__ __forceinline__ void key_corner(const Key128& k, int Lc, uint32_t c[3
     c[2] = compact3(k.hi) << lo | compact3(k.lo);
 }
 
-// One slot per calling thread from a global counter, one atomic per group of converged threads.
-template <class T>
-__device__ __forceinline__ T claim(T* ctr) {
-    cg::coalesced_group grp = cg::coalesced_threads();
-    T base = 0;
-    if (grp.thread_rank() == 0) base = atomicAdd(ctr, (T)grp.size());
-    return grp.shfl(base, 0) + (T)grp.thread_rank();
-}
-
-// One thread per entry of every table in `in` (nodes of depth d).  An entry resolves kWideLv levels below its node:
-// at sub-level k it lies in the cell of level d + k + 1 whose node has depth d + k.  That cell ends the walk when it
-// is a leaf or when d + k >= max_depth; it is then emitted (count mode: tallied in hist) by the first of the
-// 8^(kWideLv-1-k) entries it covers.  An entry that never ends is the table id of a node of depth d + kWideLv, which
-// joins the next frontier.  The root table of wide_p = v sits at depth -v; its first v levels are the virtual
-// root's octant 0, so only entries with zero virtual bits are real.
-template <class K, bool kCount>
-__global__ void __launch_bounds__(kTB) wire_expand_kernel(const uint32_t* __restrict__ wide, const WireNode* __restrict__ in,
-                                                          long long n_in, int d, int v, int max_depth, int Lc,
-                                                          WireNode* __restrict__ next, unsigned int* __restrict__ n_next,
-                                                          K* __restrict__ keys, uint8_t* __restrict__ lvls,
-                                                          unsigned long long* __restrict__ n_cells,
-                                                          unsigned long long* __restrict__ hist) {
-    constexpr int LV = kWideLv;
-    constexpr uint32_t M = (1u << LV) - 1u;
-    __shared__ unsigned int tally[2 * kWireLevels];   // count mode: leaves, then internal cells, by level
-    if (kCount) {
-        for (int i = threadIdx.x; i < 2 * kWireLevels; i += blockDim.x) tally[i] = 0;
-        __syncthreads();
+// The sink of the fill: each emitted cell's key, its corner left-aligned to Lc bits, and its level.
+template <class K>
+struct WireKeys {
+    static constexpr bool kCount = false;
+    K* keys;
+    uint8_t* lvls;
+    unsigned long long* n_cells;
+    int Lc;
+    __device__ __forceinline__ void operator()(uint32_t, uint32_t, int L, uint32_t x, uint32_t y, uint32_t z) const {
+        const int up = Lc - L;
+        const uint32_t c[3] = {x << up, y << up, z << up};
+        const unsigned long long s = wire_claim(n_cells);
+        make_key(keys[s], c, Lc);
+        lvls[s] = (uint8_t)L;
     }
-    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long f = g >> (3 * LV);
-    const uint32_t e = (uint32_t)(g & (kWideEntries - 1));
-    const int k0 = d < 0 ? -d : 0;
-    const uint32_t ex = (e >> (2 * LV)) & M, ey = (e >> LV) & M, ez = e & M;
-    if (f < n_in && ((ex | ey | ez) >> (LV - k0)) == 0) {
-        const WireNode F = in[f];
-        const uint32_t w = wide[(size_t)F.table * kWideEntries + e];
-        // leaf word: bits 23..30 hold 103 + leaf level + v (build_wide_kernel)
-        const int leaf_lvl = (w & kLeafBit) ? (int)((w >> 23) & 0xffu) - 103 - v : -1;
-        bool inner = true;
-        for (int k = k0; k < LV; ++k) {
-            const int dn = d + k, sh = LV - 1 - k;
-            const bool first = ((ex | ey | ez) & ((1u << sh) - 1u)) == 0u;
-            if (leaf_lvl == dn + 1 || dn >= max_depth) {
-                if (first) {
-                    if (kCount) {
-                        atomicAdd(&tally[dn + 1], 1u);
-                    } else {
-                        const int L = dn + 1, up = Lc - L;
-                        const uint32_t c[3] = {((F.x << (k + 1)) | (ex >> sh)) << up, ((F.y << (k + 1)) | (ey >> sh)) << up,
-                                               ((F.z << (k + 1)) | (ez >> sh)) << up};
-                        const unsigned long long s = claim(n_cells);
-                        make_key(keys[s], c, Lc);
-                        lvls[s] = (uint8_t)L;
-                    }
-                }
-                inner = false;
-                break;
-            }
-            if (kCount && first) atomicAdd(&tally[kWireLevels + dn + 1], 1u);
-        }
-        if (inner) {
-            const unsigned int s = claim(n_next);
-            next[s] = WireNode{w, (F.x << LV) | ex, (F.y << LV) | ey, (F.z << LV) | ez};
-        }
-    }
-    if (kCount) {
-        __syncthreads();
-        for (int i = threadIdx.x; i < 2 * kWireLevels; i += blockDim.x)
-            if (tally[i]) atomicAdd(hist + i, (unsigned long long)tally[i]);
-    }
-}
+};
 
 // Vertex order inside a cell: for each (a, b) in (0,0), (0,1), (1,0), (1,1), the x-, y- and z-parallel edges whose two
 // other corner selectors, in axis order, are (a, b); each edge from its low to its high end.  Bit v of
@@ -183,7 +119,7 @@ struct WireXf {
 // contiguous run.  Bounds follow the reference's float expression ((float)i / gridsz - offset) / scale, each
 // operation rounded to nearest.
 template <class K>
-__global__ void __launch_bounds__(kTB) wire_write_kernel(const K* __restrict__ keys, const uint8_t* __restrict__ lvls,
+__global__ void __launch_bounds__(kWireTB) wire_write_kernel(const K* __restrict__ keys, const uint8_t* __restrict__ lvls,
                                                          long long n, int Lc, WireXf xf, float* __restrict__ out) {
     __shared__ float bb[kWriteCells][6];
     const long long c0 = (long long)blockIdx.x * kWriteCells;
@@ -217,19 +153,14 @@ __global__ void __launch_bounds__(kTB) wire_write_kernel(const K* __restrict__ k
     }
 }
 
-unsigned int blocks_for(long long threads) { return (unsigned int)((threads + kTB - 1) / kTB); }
-
 int clamp_depth(int max_depth) { return std::min(std::max(max_depth, 0), kWireLevels - 2); }
 
 template <class K>
 cudaError_t fill_impl(const WireTree& t, const WireLevels& lv, int mm, int Lc, long long n, float* out, cudaStream_t s,
                       int* launches) {
-    long long cap = 1;   // frontier size: the most nodes of any depth the walk visits
-    for (int l = 1; l <= mm; ++l) cap = std::max(cap, lv.inner[l]);
     K* keys[2] = {nullptr, nullptr};
     uint8_t* lvls[2] = {nullptr, nullptr};
-    WireNode* nodes[2] = {nullptr, nullptr};
-    unsigned long long* ctr = nullptr;   // {cells, next frontier}
+    unsigned long long* n_cells = nullptr;
     void* tmp = nullptr;
     size_t tmp_bytes = 0;
     cudaError_t e = cudaSuccess;
@@ -239,28 +170,10 @@ cudaError_t fill_impl(const WireTree& t, const WireLevels& lv, int mm, int Lc, l
     for (int i = 0; i < 2; ++i) {
         alloc((void**)&keys[i], (size_t)n * sizeof(K));
         alloc((void**)&lvls[i], (size_t)n);
-        alloc((void**)&nodes[i], (size_t)cap * sizeof(WireNode));
     }
-    alloc((void**)&ctr, 2 * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMemsetAsync(ctr, 0, 2 * sizeof(unsigned long long), s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(nodes[0], 0, sizeof(WireNode), s);   // the root: table 0, corner 0
-    long long n_in = 1;
-    int cur = 0;
-    for (int d = -t.wide_p; e == cudaSuccess; d += kWideLv) {
-        if (d > 0) {
-            if (d > mm) break;
-            n_in = lv.inner[d];
-            if (n_in == 0) break;
-            e = cudaMemsetAsync(ctr + 1, 0, sizeof(unsigned long long), s);
-        }
-        if (e != cudaSuccess) break;
-        wire_expand_kernel<K, false><<<blocks_for(n_in * kWideEntries), kTB, 0, s>>>(
-            t.wide, nodes[cur], n_in, d, t.wide_p, mm, Lc, nodes[cur ^ 1], reinterpret_cast<unsigned int*>(ctr + 1),
-            keys[0], lvls[0], ctr, nullptr);
-        e = cudaGetLastError();
-        ++*launches;
-        cur ^= 1;
-    }
+    alloc((void**)&n_cells, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMemsetAsync(n_cells, 0, sizeof(unsigned long long), s);
+    if (e == cudaSuccess) e = wire_walk(t, lv, mm, WireKeys<K>{keys[0], lvls[0], n_cells, Lc}, s, launches);
     if (e == cudaSuccess) {
         if constexpr (std::is_same<K, unsigned long long>::value) {
             e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys[0], keys[1], lvls[0], lvls[1], (int)n, 0, 3 * Lc, s);
@@ -278,12 +191,12 @@ cudaError_t fill_impl(const WireTree& t, const WireLevels& lv, int mm, int Lc, l
     if (e == cudaSuccess) {
         WireXf xf;
         for (int a = 0; a < 3; ++a) { xf.offset[a] = t.offset[a]; xf.scale[a] = t.scale[a]; }
-        wire_write_kernel<K><<<(unsigned int)((n + kWriteCells - 1) / kWriteCells), kTB, 0, s>>>(keys[1], lvls[1], n, Lc, xf, out);
+        wire_write_kernel<K><<<(unsigned int)((n + kWriteCells - 1) / kWriteCells), kWireTB, 0, s>>>(keys[1], lvls[1], n, Lc, xf, out);
         e = cudaGetLastError();
         ++*launches;
     }
-    for (int i = 0; i < 2; ++i) { cudaFreeAsync(keys[i], s); cudaFreeAsync(lvls[i], s); cudaFreeAsync(nodes[i], s); }
-    cudaFreeAsync(ctr, s);
+    for (int i = 0; i < 2; ++i) { cudaFreeAsync(keys[i], s); cudaFreeAsync(lvls[i], s); }
+    cudaFreeAsync(n_cells, s);
     cudaFreeAsync(tmp, s);
     return e;
 }
@@ -310,8 +223,8 @@ cudaError_t wire_levels(const WireTree& t, WireLevels& L, cudaStream_t s, int* l
     for (int d = -t.wide_p; e == cudaSuccess && n_in > 0; d += kWideLv) {
         e = cudaMemsetAsync(n_next, 0, sizeof(unsigned int), s);
         if (e != cudaSuccess) break;
-        wire_expand_kernel<unsigned long long, true><<<blocks_for(n_in * kWideEntries), kTB, 0, s>>>(
-            t.wide, nodes[cur], n_in, d, t.wide_p, INT_MAX, 0, nodes[cur ^ 1], n_next, nullptr, nullptr, nullptr, hist);
+        wire_expand_kernel<WireCount><<<wire_blocks(n_in * kWideEntries), kWireTB, 0, s>>>(
+            t.wide, nodes[cur], n_in, d, t.wide_p, INT_MAX, nodes[cur ^ 1], n_next, WireCount{hist});
         e = cudaGetLastError();
         ++*launches;
         unsigned int h = 0;

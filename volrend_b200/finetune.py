@@ -5,6 +5,7 @@
                                     [--step_size S] [--sigma_thresh S] [--stop_thresh S] [--background B]
                                     [--steps 100] [--lr 1e-2] [--batch 4] [--seed 0] [--holdout K]
                                     [--refine-every K] [--refine-fraction 0.1] [--max-depth 23]
+                                    [--tv-sigma 0] [--tv-color 0]
 
 The fit uses the march's own samples: the renders are ``render_batch``'s float output and the gradients come from the
 same samples on the GPU (``vr_tree_leaf_grads``, see :func:`volrend_b200.leaf_grads`; formulas in DESIGN.md section
@@ -12,7 +13,9 @@ same samples on the GPU (``vr_tree_leaf_grads``, see :func:`volrend_b200.leaf_gr
 renders a batch of views, takes the MSE on RGB against the targets, back-propagates it to the leaves, takes one Adam
 step on the master and writes it, rounded to fp16, into the device tree (``N3Tree.update_data``).  The structure
 changes only with ``--refine-every K``: every K steps the leaves that carry the most residual error are split
-(coarse-to-fine, :mod:`volrend_b200.refine`, DESIGN.md section 19).  Columns the device does not keep (coefficients of a basis size without its own kernel beyond the first, and
+(coarse-to-fine, :mod:`volrend_b200.refine`, DESIGN.md section 19).  ``--tv-sigma`` / ``--tv-color`` add a
+total-variation prior between neighbouring leaves to the gradient (:func:`volrend_b200.leaf_tv`, DESIGN.md section 20),
+which keeps the many small leaves of a refined tree from fitting each training ray on its own.  Columns the device does not keep (coefficients of a basis size without its own kernel beyond the first, and
 SG / ASG lobes) get no gradient and keep their values.
 
 Targets are one PNG per pose or one ``.npy`` of shape [V, H, W, 3 | 4], uint8 or float in [0, 1].  RGBA targets are
@@ -47,7 +50,8 @@ def _target_rgb(img, background: float, device):
 
 
 def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int, seed: int, on_step=None,
-             refine_every: int = 0, refine_fraction: float = 0.1, max_depth: int = 23, on_refine=None):
+             refine_every: int = 0, refine_fraction: float = 0.1, max_depth: int = 23, on_refine=None,
+             tv_sigma: float = 0.0, tv_color: float = 0.0):
     """Fits the leaf data of ``tree`` (an ``N3Tree`` loaded with ``load_cuda(slot_map=True)`` that still holds its host
     data) to ``targets``: a sequence of one image per camera in ``cams`` ([H, W, 3 | 4], uint8 or float, indexed
     lazily, so it may read files on demand).  Each of ``steps`` steps takes the next ``batch`` views of a shuffle seeded
@@ -61,14 +65,23 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
     :func:`volrend_b200.refine_plan` (``refine_fraction``, ``max_depth``); the master and both Adam moments are
     gathered by its ``src`` (a new slot starts with its parent's value and moments, the step count carries on), the
     device tree is re-created with the slot map from ``master.half()`` and ``on_refine(step, n_split, nodes_before,
-    nodes_after)`` is called.  ``tree`` (``child_``, ``capacity``) then describes the refined tree."""
+    nodes_after)`` is called.  ``tree`` (``child_``, ``capacity``) then describes the refined tree.
+
+    Total variation: with ``tv_sigma`` or ``tv_color`` > 0, every step adds the gradient of the TV prior of the master
+    (:func:`volrend_b200.leaf_tv`, weights ``tv_sigma`` for sigma and ``tv_color`` for the colour coefficients) to the
+    image gradient before the Adam step.  The neighbour table (:func:`volrend_b200.leaf_neighbors`) is built before
+    the first step and again after every refinement that splits leaves.  ``losses`` and ``on_step`` stay the MSE."""
     import torch
-    from .host import leaf_grads, render_batch
+    from .host import leaf_grads, leaf_neighbors, leaf_tv, render_batch
     from .refine import leaf_scores, refine_plan
     if steps < 0 or batch < 1:
         raise ValueError(f"steps {steps} must be >= 0 and batch {batch} >= 1")
     if refine_every < 0:
         raise ValueError(f"refine_every {refine_every} must be >= 0")
+    for name, w in (("tv_sigma", tv_sigma), ("tv_color", tv_color)):
+        if not (float(w) >= 0.0) or math.isinf(float(w)):
+            raise ValueError(f"{name} {w} must be finite and >= 0")
+    tv = tv_sigma > 0 or tv_color > 0
     if len(targets) != len(cams):
         raise ValueError(f"{len(targets)} targets for {len(cams)} views")
     if not cams:
@@ -85,6 +98,8 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
     fo = torch.empty((nb, H, W, 4), dtype=torch.float32, device=dev)
     dpix = torch.zeros((nb, H, W, 4), dtype=torch.float32, device=dev)
     grad = torch.zeros_like(master)
+    nbr = leaf_neighbors(tree) if tv and steps > 0 else None
+    tv_energy = torch.zeros(1, dtype=torch.float64, device=dev) if tv else None
     losses = []
     for step in range(steps):
         if refine_every > 0 and step > 0 and step % refine_every == 0:
@@ -99,6 +114,8 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
                 tree.data_ = master.detach().half().cpu().numpy()
                 tree.load_cuda(slot_map=True)
                 tree.clear_cpu_memory()
+                if tv:
+                    nbr = leaf_neighbors(tree)
             if on_refine is not None:
                 on_refine(step, n1 - n0, n0, n1)
         if pos + nb > len(cams):
@@ -115,6 +132,8 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
         dpix[..., :3] = diff * (2.0 / diff.numel())
         grad.zero_()
         leaf_grads(tree, vc, options, dpix, out=grad)
+        if tv:
+            leaf_tv(tree, nbr, master.detach(), tv_sigma, tv_color, out=grad, energy=tv_energy)
         master.grad = grad
         opt.step()
         tree.update_data(master.detach())
@@ -229,6 +248,10 @@ def _parser() -> argparse.ArgumentParser:
                     help="share of the candidate leaves split at each refinement, in [0, 1]")
     ap.add_argument("--max-depth", type=int, default=23,
                     help="leaves at this depth (root's slots = 1) or deeper are not split (at most 23)")
+    ap.add_argument("--tv-sigma", type=float, default=0.0,
+                    help="weight of the total-variation prior on sigma between neighbouring leaves (0: none)")
+    ap.add_argument("--tv-color", type=float, default=0.0,
+                    help="weight of the total-variation prior on the colour coefficients (0: none)")
     return ap
 
 
@@ -261,6 +284,9 @@ def main(argv=None) -> int:
         ap.error(f"--refine-fraction {args.refine_fraction} must be in [0, 1]")
     if args.max_depth < 1:
         ap.error(f"--max-depth {args.max_depth} < 1")
+    for flag, w in (("--tv-sigma", args.tv_sigma), ("--tv-color", args.tv_color)):
+        if not (w >= 0.0) or math.isinf(w):
+            ap.error(f"{flag} {w} must be a finite number >= 0")
     if os.path.abspath(args.input) == os.path.abspath(args.output):
         ap.error("the output would overwrite the input")
     for p in [args.input] + args.targets:
@@ -295,7 +321,7 @@ def main(argv=None) -> int:
                          steps=args.steps, lr=args.lr, batch=args.batch, seed=args.seed,
                          on_step=lambda s, l: print(f"step {s}: loss {l:.6g}"),
                          refine_every=args.refine_every, refine_fraction=args.refine_fraction,
-                         max_depth=args.max_depth,
+                         max_depth=args.max_depth, tv_sigma=args.tv_sigma, tv_color=args.tv_color,
                          on_refine=lambda s, n, a, b: print(f"refine before step {s}: split {n}, nodes {a} -> {b}"))
     if held:
         print(f"held-out PSNR after: {_psnr(tree, cams, targets, held, opt):.3f} dB")

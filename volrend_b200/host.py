@@ -777,6 +777,72 @@ def leaf_grads(tree: N3Tree, cams, options: RenderOptions, dpix, out=None, float
     return out
 
 
+def _tv_tree(tree: N3Tree, what: str):
+    import torch
+    if not tree.is_cuda_loaded():
+        raise RuntimeError("N3Tree is not loaded on the device")
+    if not tree._slot_map:
+        raise RuntimeError(f"{what} needs the slot map: load the tree with load_cuda(slot_map=True)")
+    return torch.device("cuda", tree._device)
+
+
+def _check_tensor(name: str, t, dtype, n: int, dev) -> None:
+    import torch
+    if (not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != dev or not t.is_contiguous()
+            or t.numel() != n):
+        raise ValueError(f"{name} must be a contiguous {str(dtype).replace('torch.', '')} tensor of {n} elements "
+                         f"on {dev}")
+
+
+def leaf_neighbors(tree: N3Tree, out=None, stream=None):
+    """Forward neighbour of every leaf slot along x, y and z (vr_tree_leaf_neighbors): a CUDA int32 tensor
+    ``[capacity * 8, 3]`` holding, for a reachable leaf slot at depth d with integer cell i, the slot of the leaf whose
+    cell holds the point (i + e_a) 2^-d of the tree's unit cube, or -1 where i_a + 1 = 2^d; internal, free and
+    unreachable slots hold -1.  ``out``: that many int32 elements on the tree's device, overwritten.  Asynchronous on
+    ``stream`` (the first call for a tree counts its cells and synchronises it).  The tree must be loaded with
+    ``load_cuda(slot_map=True)``; a structural change (a new ``load_cuda``) needs a new table."""
+    import torch
+    dev = _tv_tree(tree, "leaf_neighbors")
+    n = tree.capacity * tree.N ** 3
+    if out is None:
+        out = torch.empty((n, 3), dtype=torch.int32, device=dev)
+    else:
+        _check_tensor("out", out, torch.int32, n * 3, dev)
+    check(lib().vr_tree_leaf_neighbors(tree._handle, out.data_ptr(), _stream_ptr(stream)))
+    return out
+
+
+def leaf_tv(tree: N3Tree, nbr, data, lambda_sigma: float, lambda_color: float, out=None, energy=None, stream=None):
+    """Total variation between neighbouring leaves (vr_tree_leaf_tv, DESIGN.md section 20) of the float32 rows ``data``
+    (``[capacity, 2, 2, 2, data_dim]`` or as many elements, e.g. the fp32 master of :func:`volrend_b200.finetune`):
+    ``E = sum_G lambda_G / N_leaf * sum_leaf sum_{c in G} sqrt(1e-8 + sum_a (v[n_a, c] - v[s, c])^2)`` over sigma and
+    the colour columns :func:`leaf_grads` writes, ``nbr`` being :func:`leaf_neighbors` of the tree.  dE/d``data`` is
+    added to ``out`` (``leaf_grads``' shape; without it a new tensor starts at 0) and E to ``energy`` (a float64 CUDA
+    tensor of one element; without it a new one starts at 0).  Returns ``(out, energy)``.  Weights must be finite and
+    >= 0; a weight of 0 skips its group.  Asynchronous on ``stream``; the gradient sums are atomic, so they vary in the
+    last bits from run to run."""
+    import torch
+    dev = _tv_tree(tree, "leaf_tv")
+    n_slots = tree.capacity * tree.N ** 3
+    n = n_slots * tree.data_dim
+    for name, w in (("lambda_sigma", lambda_sigma), ("lambda_color", lambda_color)):
+        if not (float(w) >= 0.0) or float(w) == float("inf"):
+            raise ValueError(f"{name} {w} must be finite and >= 0")
+    _check_tensor("nbr", nbr, torch.int32, n_slots * 3, dev)
+    _check_tensor("data", data, torch.float32, n, dev)
+    if out is None:
+        out = torch.zeros((tree.capacity, tree.N, tree.N, tree.N, tree.data_dim), dtype=torch.float32, device=dev)
+    else:
+        _check_tensor("out", out, torch.float32, n, dev)
+    if energy is None:
+        energy = torch.zeros(1, dtype=torch.float64, device=dev)
+    else:
+        _check_tensor("energy", energy, torch.float64, 1, dev)
+    check(lib().vr_tree_leaf_tv(tree._handle, nbr.data_ptr(), data.data_ptr(), float(lambda_sigma),
+                                float(lambda_color), out.data_ptr(), energy.data_ptr(), _stream_ptr(stream)))
+    return out, energy
+
+
 def _draw_probe_runs(tree: N3Tree, arr, options, oarr, tile, img, fo, s) -> None:
     """The probe discs of a batch rendered with options per view (``arr`` cameras, ``oarr`` their vr_options): one
     vr_draw_probe per run of consecutive views with the same probe settings."""
