@@ -203,6 +203,16 @@ def test_slot_map_flag(built):
     assert lib().vr_tree_leaf_weights(plain._handle, C.byref(c), 1, C.byref(o), None, w.data_ptr(), None, None,
                                       None) == _capi.VR_EUNSUPPORTED
     assert b"slot map" in lib().vr_last_error()
+    # host memory in any of the buffers is refused before a launch: the device buffer stays as it was
+    host, cnt = np.zeros(st.capacity * 8, np.float32), np.zeros(5, np.int64)
+    for name, bufs in ((b"weight_dev", (host.ctypes.data, None, None)),
+                       (b"alpha_dev", (w.data_ptr(), host.ctypes.data, None)),
+                       (b"counters_dev", (w.data_ptr(), None, cnt.ctypes.data))):
+        assert lib().vr_tree_leaf_weights(mapped._handle, C.byref(c), 1, C.byref(o), None, *bufs,
+                                          None) == _capi.VR_EINVAL
+        assert name in lib().vr_last_error()
+    torch.cuda.synchronize()
+    assert not w.any() and not host.any()
     h = C.c_void_p()
     d, keep = plain._plain_desc()
     assert lib().vr_tree_create_ex(C.byref(d), 2, C.byref(h)) == _capi.VR_EINVAL and not h.value

@@ -204,6 +204,10 @@ def test_refusals(built):
                                 None) == _capi.VR_EINVAL
     assert L.vr_tree_leaf_error(tree._handle, arr, 2, C.byref(o), None, err.data_ptr(), host.ctypes.data, None,
                                 None) == _capi.VR_EINVAL
+    cnt = np.zeros(5, np.int64)
+    assert L.vr_tree_leaf_error(tree._handle, arr, 2, C.byref(o), None, err.data_ptr(), s.data_ptr(), cnt.ctypes.data,
+                                None) == _capi.VR_EINVAL
+    assert b"counters_dev" in L.vr_last_error()
     assert not s.any()
     with pytest.raises(ValueError, match="err"):
         leaf_error(tree, cams, RenderOptions(), err[:1])

@@ -246,10 +246,10 @@ def test_cli_argument_errors(tmp_path, capsys):
     assert not (tmp_path / "o.npz").exists()
 
 
-def test_png_targets_read_lazily_and_composited(tmp_path):
+def test_view_png_targets_read_lazily_and_composited(tmp_path):
     import torch
     from volrend_b200 import write_png_file
-    from volrend_b200.finetune import _target_rgb, read_targets
+    from volrend_b200.views import read_targets, target_rgb
     rgba = np.zeros((4, 5, 4), np.uint8)
     rgba[..., 0] = 255
     rgba[..., 3] = np.arange(5, dtype=np.uint8) * 60
@@ -259,7 +259,7 @@ def test_png_targets_read_lazily_and_composited(tmp_path):
     assert len(t) == 2 and len(t[:1]) == 1
     img = t[1]
     assert img.shape == (4, 5, 4) and np.array_equal(img, rgba)
-    rgb = _target_rgb(img, 0.25, torch.device("cpu")).numpy()
+    rgb = target_rgb(img, 0.25, torch.device("cpu")).numpy()
     a = rgba[..., 3:4] / 255.0
     np.testing.assert_allclose(rgb, np.concatenate([a + 0.25 * (1 - a), 0.25 * (1 - a), 0.25 * (1 - a)], -1), atol=1e-6)
 

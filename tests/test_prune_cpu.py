@@ -167,16 +167,16 @@ def test_cli_argument_errors(tmp_path, capsys):
     assert not (tmp_path / "o.npz").exists()
 
 
-def test_pose_and_intrinsics_files(tmp_path):
-    from volrend_b200 import prune
+def test_view_pose_and_intrinsics_files(tmp_path):
+    from volrend_b200 import views
     p = tmp_path / "two.txt"
     m = np.arange(32, dtype=np.float32).reshape(2, 4, 4)
     p.write_text("\n".join(" ".join(str(v) for v in r) for r in m.reshape(8, 4)))
-    got = prune.read_poses(str(p))
+    got = views.read_poses(str(p))
     assert len(got) == 2 and np.array_equal(np.stack(got), m)
     k = tmp_path / "k.txt"
     k.write_text("500 0 400 0\n0 510 400 0\n0 0 1 0\n0 0 0 1\n")
-    assert prune.read_intrinsics(str(k)) == (500.0, 510.0)
+    assert views.read_intrinsics(str(k)) == (500.0, 510.0)
 
 
 def test_new_entry_points_without_a_device(built):

@@ -60,7 +60,8 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     import torch
-    from volrend_b200 import Camera, N3Tree, RenderOptions, leaf_grads, render_batch, synth
+    from volrend_b200 import N3Tree, RenderOptions, leaf_grads, render_batch, synth
+    from volrend_b200.views import cameras
     if not torch.cuda.is_available():
         raise SystemExit("finetune_bench needs a CUDA device")
     c = card()
@@ -70,11 +71,7 @@ def main():
     print(f"tree built in {time.time() - t0:.1f} s: capacity {st.capacity}", flush=True)
     free0 = torch.cuda.mem_get_info()[0]
     f = synth.focal_for(W)
-    cams = []
-    for p in synth.nerf_synthetic_test_poses(200):
-        cam = Camera(W, H, f, f)
-        cam.set_c2w(p)
-        cams.append(cam)
+    cams = cameras(synth.nerf_synthetic_test_poses(200), W, H, f, f)
     opt = RenderOptions()
     tree = N3Tree()
     tree.load_npz(st.npz_dict())

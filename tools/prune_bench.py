@@ -68,8 +68,9 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     import torch
-    from volrend_b200 import Camera, N3Tree, RenderOptions, compress_npz, leaf_weights, prune_npz, render_batch, synth
+    from volrend_b200 import N3Tree, RenderOptions, compress_npz, leaf_weights, prune_npz, render_batch, synth
     from volrend_b200.compress import _write_npz
+    from volrend_b200.views import cameras
     c = card()
     print("card:", c, flush=True)
     t0 = time.time()
@@ -77,17 +78,9 @@ def main():
     z = st.npz_dict()
     print(f"tree built in {time.time() - t0:.1f} s: capacity {st.capacity}", flush=True)
     f = synth.focal_for(W)
-
-    def cams_of(poses):
-        out = []
-        for p in poses:
-            cam = Camera(W, H, f, f)
-            cam.set_c2w(p)
-            out.append(cam)
-        return out
-
-    cams = cams_of(synth.nerf_synthetic_test_poses(200))
-    held = cams_of(synth.nerf_synthetic_test_poses(400)[1::2][:: max(1, 200 // args.psnr_views)][:args.psnr_views])
+    cams = cameras(synth.nerf_synthetic_test_poses(200), W, H, f, f)
+    held = cameras(synth.nerf_synthetic_test_poses(400)[1::2][:: max(1, 200 // args.psnr_views)][:args.psnr_views],
+                   W, H, f, f)
     opt = RenderOptions()
     imgs = torch.empty((200, H, W, 4), dtype=torch.uint8, device="cuda")
 

@@ -38,19 +38,16 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     import torch
-    from volrend_b200 import (Camera, N3Tree, RenderOptions, leaf_error, leaf_grads, leaf_neighbors, leaf_tv,
-                              refine_plan, render_batch, synth)
+    from volrend_b200 import (N3Tree, RenderOptions, leaf_error, leaf_grads, leaf_neighbors, leaf_tv, refine_plan,
+                              render_batch, synth)
+    from volrend_b200.views import cameras
     if not torch.cuda.is_available():
         raise SystemExit("tv_bench needs a CUDA device")
     c = card()
     print("card:", c, flush=True)
     st = synth.make_tree("lego", depth=args.depth, basis_dim=16, seed=0)
     f = synth.focal_for(W)
-    cams = []
-    for p in synth.nerf_synthetic_test_poses(200):
-        cam = Camera(W, H, f, f)
-        cam.set_c2w(p)
-        cams.append(cam)
+    cams = cameras(synth.nerf_synthetic_test_poses(200), W, H, f, f)
     opt = RenderOptions()
     dd = st.data_dim
 

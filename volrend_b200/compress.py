@@ -27,6 +27,23 @@ ROWS = 65536
 DROPPED_KEYS = ("parent_depth", "geom_resize_fact", "n_free", "n_internal", "depth_limit")
 
 
+def carried_keys(z, replaced=()) -> list:
+    """The keys of the tree dict ``z`` (``N3Tree`` npz keys) that a rewrite of it carries over unchanged: all but the
+    ``replaced`` ones and DROPPED_KEYS."""
+    return [k for k in (z.files if hasattr(z, "files") else z) if k not in replaced and k not in DROPPED_KEYS]
+
+
+def check_uncompressed(z, advice: str) -> None:
+    """Raises ValueError unless the tree dict ``z`` holds the uncompressed ``child`` and ``data`` arrays that pruning,
+    refinement and fine-tuning rewrite; ``advice`` says in which order to run the tools instead."""
+    keys = z.files if hasattr(z, "files") else z
+    if "quant_map" in keys or "quant_colors" in keys:
+        raise ValueError(f"the tree is already compressed (quant_map): {advice}")
+    for k in ("child", "data"):
+        if k not in keys:
+            raise ValueError(f"the tree has no '{k}' array")
+
+
 def compress_device(data, data_dim: int, sigma_thresh: float = 2.0, retain: int = 1, bits: int = 16, stream=None):
     """``vr_tree_compress`` on a CUDA tensor ``data`` (fp16 or int16 bits, [n_child, data_dim] or any shape with
     that many elements).  Returns device int16 tensors (fp16 bits) ``(quant_colors [n_quant, 65536, 3], quant_map
@@ -96,7 +113,7 @@ def compress_npz(z, *, bits: int = 16, sigma_thresh: float = 2.0, retain: int = 
     shape = data.shape[:-1]
     flat = np.ascontiguousarray(data).view(np.uint16).reshape(-1, data_dim)
     colors, qmap, sigma, retained, _ = (backend or compress_arrays)(flat, data_dim, sigma_thresh, retain, bits)
-    out = {k: v for k, v in z.items() if k != "data" and k not in DROPPED_KEYS}
+    out = {k: z[k] for k in carried_keys(z, ("data",))}
     out["quant_colors"] = colors.view(np.float16).reshape(-1, ROWS, 3)
     out["quant_map"] = qmap.reshape((-1,) + shape)
     out["sigma"] = sigma.view(np.float16).reshape(shape)
@@ -157,7 +174,7 @@ def main(argv=None) -> int:
             d = {k: z[k] for k in z.files}
         try:
             if args.noquant:
-                d = {k: v for k, v in d.items() if k not in DROPPED_KEYS}
+                d = {k: d[k] for k in carried_keys(d)}
             else:
                 d = compress_npz(d, bits=args.bits, sigma_thresh=args.sigma_thresh, retain=args.retain)
         except (ValueError, VolrendError) as e:

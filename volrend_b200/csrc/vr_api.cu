@@ -73,6 +73,11 @@ int vrb::buffer_check(const vr_tree* t, const void* p, const char* what) {
     return VR_OK;
 }
 
+int vrb::need_slot_map(const vr_tree* t, const char* what) {
+    if (t->wslot) return VR_OK;
+    return fail(VR_EUNSUPPORTED, "%s needs the slot map: create the tree with VR_TREE_SLOT_MAP", what);
+}
+
 namespace {
 // f(std::integral_constant<int, K>{}) for the kernel bases K the march kernels are built for (kbd_built); `otherwise`
 // for any other kbd.
@@ -300,6 +305,32 @@ int render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views,
     if (n_views > 0 && (!rgba8_dev || !depth_dev)) return fail(VR_EINVAL, "composite mode needs colour and depth inputs");
     return render_batch(t, cams, n_views, opt, opt_stride, tile, rgba8_dev, rgba32f_dev, nullptr, stream, depth_dev);
 }
+
+// A buffer of a leaf pass, its name in the errors, and whether the pass needs it.
+struct PassBuf { const void* p; const char* name; bool required = false; };
+
+// The march-based leaf passes (vr_tree_leaf_weights, _error, _grads), `what` naming the pass.  The checks run in this
+// order: a required buffer that is NULL is VR_EINVAL; check_batch (an empty batch is VR_OK before any pointer is
+// read); `refuse(opt)`, the pass's own refusals; the slot map; buffer_check of every buffer; an empty rect is VR_OK.
+// P holds the pass's buffers; the rect, the slot map and the gradient row width are added here.
+int leaf_pass(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt, const vr_rect* tile,
+              void* stream, Pass pass, const char* what, LaunchDev P, std::initializer_list<PassBuf> bufs,
+              int (*refuse)(const vr_options*) = nullptr) {
+    if (n_views > 0)
+        for (const PassBuf& b : bufs)
+            if (b.required && !b.p) return fail(VR_EINVAL, "%s: null %s", what, b.name);
+    vr_rect r;
+    int rc = check_batch(t, cams, n_views, opt, tile, r);
+    if (rc || n_views == 0) return rc;
+    if ((refuse && (rc = refuse(opt))) || (rc = need_slot_map(t, what))) return rc;
+    for (const PassBuf& b : bufs)
+        if ((rc = buffer_check(t, b.p, b.name))) return rc;
+    if (r.w == 0 || r.h == 0) return VR_OK;
+    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
+    P.wslot = t->wslot;
+    P.grad_dim = t->data_dim;
+    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, pass);
+}
 }  // namespace
 
 // vr_render_batch (opt_stride 0: one options struct for every view) and vr_render_batch_opts (opt_stride 1: view i
@@ -365,57 +396,33 @@ int vr_render_batch_opts(const vr_tree* t, const vr_camera* cams, int n_views, c
 int vr_tree_leaf_weights(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
                          const vr_rect* tile, float* weight_dev, float* alpha_dev, vr_counters* counters_dev,
                          void* stream) {
-    if (n_views > 0 && !weight_dev) return fail(VR_EINVAL, "null weight buffer");
-    vr_rect r;
-    const int rc = check_batch(t, cams, n_views, opt, tile, r);
-    if (rc || n_views == 0) return rc;
-    if (!t->wslot)
-        return fail(VR_EUNSUPPORTED, "leaf weights need the slot map: create the tree with VR_TREE_SLOT_MAP");
-    if (r.w == 0 || r.h == 0) return VR_OK;
     LaunchDev P{};
-    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
-    P.counters = counters_dev;
-    P.wslot = t->wslot; P.weights = weight_dev; P.alpha = alpha_dev;
-    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, Pass::kWeights);
+    P.weights = weight_dev; P.alpha = alpha_dev; P.counters = counters_dev;
+    return leaf_pass(t, cams, n_views, opt, tile, stream, Pass::kWeights, "vr_tree_leaf_weights", P,
+                     {{weight_dev, "weight_dev", true}, {alpha_dev, "alpha_dev"}, {counters_dev, "counters_dev"}});
 }
 
 int vr_tree_leaf_error(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
                        const vr_rect* tile, const float* err_dev, float* score_dev, vr_counters* counters_dev,
                        void* stream) {
-    if (n_views > 0 && (!err_dev || !score_dev)) return fail(VR_EINVAL, "null err or score buffer");
-    vr_rect r;
-    int rc = check_batch(t, cams, n_views, opt, tile, r);
-    if (rc || n_views == 0) return rc;
-    if (!t->wslot)
-        return fail(VR_EUNSUPPORTED, "leaf error needs the slot map: create the tree with VR_TREE_SLOT_MAP");
-    if ((rc = buffer_check(t, err_dev, "err_dev")) || (rc = buffer_check(t, score_dev, "score_dev"))) return rc;
-    if (r.w == 0 || r.h == 0) return VR_OK;
     LaunchDev P{};
-    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
-    P.counters = counters_dev;
-    P.wslot = t->wslot; P.err = err_dev; P.score = score_dev;
-    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, Pass::kError);
+    P.err = err_dev; P.score = score_dev; P.counters = counters_dev;
+    return leaf_pass(t, cams, n_views, opt, tile, stream, Pass::kError, "vr_tree_leaf_error", P,
+                     {{err_dev, "err_dev", true}, {score_dev, "score_dev", true}, {counters_dev, "counters_dev"}});
 }
 
 int vr_tree_leaf_grads(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
                        const vr_rect* tile, const float* dpix_dev, float* grad_dev, float* rgba32f_dev, void* stream) {
-    if (n_views > 0 && (!dpix_dev || !grad_dev)) return fail(VR_EINVAL, "null dpix or gradient buffer");
-    vr_rect r;
-    int rc = check_batch(t, cams, n_views, opt, tile, r);
-    if (rc || n_views == 0) return rc;
-    if (opt->render_depth) return fail(VR_EINVAL, "leaf gradients are of the colour output: render_depth is not supported");
-    if (!t->wslot)
-        return fail(VR_EUNSUPPORTED, "leaf gradients need the slot map: create the tree with VR_TREE_SLOT_MAP");
-    if ((rc = buffer_check(t, dpix_dev, "dpix_dev")) || (rc = buffer_check(t, grad_dev, "grad_dev")) ||
-        (rc = buffer_check(t, rgba32f_dev, "rgba32f_dev")))
-        return rc;
-    if (r.w == 0 || r.h == 0) return VR_OK;
     LaunchDev P{};
-    P.x0 = r.x0; P.y0 = r.y0; P.w = r.w; P.h = r.h;
+    P.dpix = reinterpret_cast<const float4*>(dpix_dev); P.grad = grad_dev;
     P.rgbaf = reinterpret_cast<float4*>(rgba32f_dev);
-    P.wslot = t->wslot;
-    P.dpix = reinterpret_cast<const float4*>(dpix_dev); P.grad = grad_dev; P.grad_dim = t->data_dim;
-    return march(t, cams, n_views, opt, 0, P, false, (cudaStream_t)stream, Pass::kGrads);
+    return leaf_pass(t, cams, n_views, opt, tile, stream, Pass::kGrads, "vr_tree_leaf_grads", P,
+                     {{dpix_dev, "dpix_dev", true}, {grad_dev, "grad_dev", true}, {rgba32f_dev, "rgba32f_dev"}},
+                     [](const vr_options* o) {
+                         return o->render_depth ? fail(VR_EINVAL, "leaf gradients are of the colour output: "
+                                                                  "render_depth is not supported")
+                                                : VR_OK;
+                     });
 }
 
 int vr_render_composite_batch(const vr_tree* t, const vr_camera* cams, int n_views, const vr_options* opt,
@@ -912,8 +919,7 @@ int vr_tree_leaf_neighbors(const vr_tree* t, int32_t* nbr_dev, void* stream_) {
     if (!t) return fail(VR_EINVAL, "null tree");
     int rc = need_device(t);
     if (rc) return rc;
-    if (!t->wslot)
-        return fail(VR_EUNSUPPORTED, "leaf neighbours need the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if ((rc = need_slot_map(t, "vr_tree_leaf_neighbors"))) return rc;
     if (!nbr_dev) return fail(VR_EINVAL, "null neighbour buffer");
     if ((rc = buffer_check(t, nbr_dev, "nbr_dev"))) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -935,8 +941,7 @@ int vr_tree_leaf_tv(const vr_tree* t, const int32_t* nbr_dev, const float* data_
     if (rc) return rc;
     if (!(lambda_sigma >= 0.f) || !(lambda_color >= 0.f) || std::isinf(lambda_sigma) || std::isinf(lambda_color))
         return fail(VR_EINVAL, "TV weights must be finite and >= 0 (sigma %g, colour %g)", lambda_sigma, lambda_color);
-    if (!t->wslot)
-        return fail(VR_EUNSUPPORTED, "leaf TV needs the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if ((rc = need_slot_map(t, "vr_tree_leaf_tv"))) return rc;
     if (!nbr_dev || !data_dev || !grad_dev) return fail(VR_EINVAL, "null neighbour, data or gradient buffer");
     if ((rc = buffer_check(t, nbr_dev, "nbr_dev")) || (rc = buffer_check(t, data_dev, "data_dev")) ||
         (rc = buffer_check(t, grad_dev, "grad_dev")) || (rc = buffer_check(t, energy_dev, "energy_dev")))

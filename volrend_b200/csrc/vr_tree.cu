@@ -479,8 +479,7 @@ int vr_tree_create_quantized(const vr_tree_quant_desc* q, vr_tree** out) { retur
 int vr_tree_update_data(vr_tree* t, const uint16_t* data_dev, void* stream) {
     if (!t) return fail(VR_EINVAL, "null tree");
     if (int rc = need_device(t)) return rc;
-    if (!t->wslot)
-        return fail(VR_EUNSUPPORTED, "updating leaf data needs the slot map: create the tree with VR_TREE_SLOT_MAP");
+    if (int rc = need_slot_map(t, "vr_tree_update_data")) return rc;
     if (!data_dev) return fail(VR_EINVAL, "null data");
     if (int rc = buffer_check(t, data_dev, "data_dev")) return rc;
     LeafSrc S{};

@@ -24,6 +24,10 @@ int need_device(const vr_tree* t);
 // device's allocation); `what` names it in the error.
 int buffer_check(const vr_tree* t, const void* p, const char* what);
 
+// The table entry -> slot map (VR_TREE_SLOT_MAP) of the operations on leaf slots: VR_EUNSUPPORTED without it; `what`
+// names the operation in the error.
+int need_slot_map(const vr_tree* t, const char* what);
+
 // A failed CUDA call: VR_ENOMEM for an allocation, else VR_ECUDA, with the message "<what>: <CUDA's text><where>".
 // The runtime's last error is cleared, so that a later launch check does not report this failure again.
 inline int cuda_fail(cudaError_t e, const char* what, const char* where = "") {

@@ -28,25 +28,14 @@ from __future__ import annotations
 
 import argparse
 import math
-import os
 import sys
 
 import numpy as np
 
-from .compress import DROPPED_KEYS, _write_npz
-from .prune import add_view_arguments, load_tree_arrays, view_setup
+from .compress import _write_npz, carried_keys, check_uncompressed
+from .views import add_view_arguments, open_inputs, target_batch
 
-
-def _target_rgb(img, background: float, device):
-    """[H, W, 3 | 4] uint8 or float -> float32 RGB on ``device``; alpha composited onto ``background``."""
-    import torch
-    t = img if isinstance(img, torch.Tensor) else torch.from_numpy(np.array(img))   # (a copy: targets may be read-only)
-    t = t.to(device=device)
-    t = t.float() / 255.0 if t.dtype == torch.uint8 else t.float()
-    if t.shape[-1] == 4:
-        a = t[..., 3:4]
-        t = t[..., :3] * a + background * (1.0 - a)
-    return t
+_ADVICE = "fine-tune the uncompressed tree first, then prune and compress"
 
 
 def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int, seed: int, on_step=None,
@@ -122,9 +111,7 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
             order, pos = gen.permutation(len(cams)), 0
         views = order[pos:pos + nb]
         pos += nb
-        tgt = torch.stack([_target_rgb(targets[int(v)], options.background_brightness, dev) for v in views])
-        if tuple(tgt.shape) != (nb, H, W, 3):
-            raise ValueError(f"targets are {tuple(tgt.shape[1:3])}, the views {H}x{W}")
+        tgt = target_batch(targets, views, options.background_brightness, dev, H, W)
         vc = [cams[int(v)] for v in views]
         render_batch(tree, vc, options, None, float_out=fo)
         diff = fo[..., :3] - tgt
@@ -164,18 +151,13 @@ def finetune_npz(z, data, *, child=None) -> dict:
     ``compress_npz`` drops are dropped, every other key passes through).  ``child``: the structure of a fit with
     refinement (``N3Tree.child_`` after :func:`finetune`), written with ``data`` of its capacity; without it the
     structure is ``z``'s.  Compressed input (``quant_map``) is refused."""
-    keys = list(z.files if hasattr(z, "files") else z)
-    if "quant_map" in keys or "quant_colors" in keys:
-        raise ValueError("the tree is compressed (quant_map): fine-tune the uncompressed tree, then prune and compress")
-    for k in ("child", "data"):
-        if k not in keys:
-            raise ValueError(f"the tree has no '{k}' array")
+    check_uncompressed(z, _ADVICE)
     src = np.asarray(z["data"])
     d = data.detach().cpu().numpy() if hasattr(data, "detach") else np.asarray(data)
     shape = src.shape if child is None else np.asarray(child).shape + src.shape[-1:]
     if d.shape != shape:
         raise ValueError(f"data has shape {d.shape}, the tree's {shape}")
-    out = {k: z[k] for k in keys if k != "data" and k not in DROPPED_KEYS}
+    out = {k: z[k] for k in carried_keys(z, ("data",))}
     out["data"] = d.astype(src.dtype)
     if child is not None:
         out["child"] = np.asarray(child, np.int32)
@@ -183,60 +165,13 @@ def finetune_npz(z, data, *, child=None) -> dict:
 
 
 # ---------------------------------------------------------------------------------------------------------- CLI
-class _PngTargets:
-    """One PNG per view, decoded when indexed."""
-
-    def __init__(self, paths):
-        self.paths = list(paths)
-
-    def __len__(self):
-        return len(self.paths)
-
-    def __getitem__(self, i):
-        if isinstance(i, slice):
-            return _PngTargets(self.paths[i])
-        from PIL import Image
-        with Image.open(self.paths[i]) as im:
-            return np.asarray(im.convert("RGBA" if im.mode in ("RGBA", "LA", "P") else "RGB"))
-
-
-def read_targets(paths, n_views: int, width: int, height: int):
-    """The targets of the CLI: one ``.npy`` [V, H, W, 3 | 4] (memory-mapped) or one PNG per view.  Raises ValueError
-    when their number or size does not match the views."""
-    if len(paths) == 1 and paths[0].endswith(".npy"):
-        t = np.load(paths[0], mmap_mode="r")
-        if t.ndim != 4 or t.shape[-1] not in (3, 4):
-            raise ValueError(f"{paths[0]} has shape {t.shape}, not [views, height, width, 3 | 4]")
-        if t.dtype != np.uint8 and not np.issubdtype(t.dtype, np.floating):
-            raise ValueError(f"{paths[0]} holds {t.dtype}, not uint8 or float")
-        n, size = t.shape[0], (t.shape[1], t.shape[2])
-        if n == n_views and size != (height, width):
-            raise ValueError(f"targets are {size[1]}x{size[0]}, the views {width}x{height}")
-    else:
-        if any(not p.lower().endswith(".png") for p in paths):
-            raise ValueError("targets are one .npy file or one .png per pose")
-        from PIL import Image
-        t, n = _PngTargets(paths), len(paths)
-        for p in paths:
-            with Image.open(p) as im:
-                if im.size != (width, height):
-                    raise ValueError(f"{p} is {im.size[0]}x{im.size[1]}, the views {width}x{height}")
-    if n != n_views:
-        raise ValueError(f"{n} targets for {n_views} poses")
-    return t
-
-
 def _parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(prog="python -m volrend_b200.finetune",
                                  description="Fine-tune the leaf values of a PlenOctree npz against images of the given "
                                              "poses (MSE on the rendered colours, Adam on the GPU).")
     ap.add_argument("input", help="npz file storing octree data (uncompressed)")
     ap.add_argument("output", help="where to write the fine-tuned npz")
-    add_view_arguments(ap)
-    ap.add_argument("--targets", nargs="+", required=True,
-                    help="one PNG per pose, or one .npy [views, height, width, 3|4] (uint8 or float in [0, 1])")
-    ap.add_argument("--background", type=float, default=1.0,
-                    help="background brightness: renders and the compositing of RGBA targets")
+    add_view_arguments(ap, targets=True)
     ap.add_argument("--steps", type=int, default=100, help="optimiser steps")
     ap.add_argument("--lr", type=float, default=1e-2, help="Adam learning rate")
     ap.add_argument("--batch", type=int, default=4, help="views per step")
@@ -261,9 +196,10 @@ def _psnr(tree, cams, targets, idx, options) -> float:
     dev = torch.device("cuda", tree._device)
     se, n = 0.0, 0
     for v in idx:
-        fo = torch.empty((1, cams[v].height, cams[v].width, 4), dtype=torch.float32, device=dev)
+        H, W = cams[v].height, cams[v].width
+        fo = torch.empty((1, H, W, 4), dtype=torch.float32, device=dev)
         render_batch(tree, [cams[v]], options, None, float_out=fo)
-        d = fo[0, ..., :3] - _target_rgb(targets[v], options.background_brightness, dev)
+        d = fo[..., :3] - target_batch(targets, [v], options.background_brightness, dev, H, W)
         se += float(d.square().sum())
         n += d.numel()
     return -10.0 * math.log10(max(se / n, 1e-30))
@@ -287,32 +223,7 @@ def main(argv=None) -> int:
     for flag, w in (("--tv-sigma", args.tv_sigma), ("--tv-color", args.tv_color)):
         if not (w >= 0.0) or math.isinf(w):
             ap.error(f"{flag} {w} must be a finite number >= 0")
-    if os.path.abspath(args.input) == os.path.abspath(args.output):
-        ap.error("the output would overwrite the input")
-    for p in [args.input] + args.targets:
-        if not os.path.exists(p):
-            ap.error(f"'{p}' does not exist")
-    poses, fx, fy = view_setup(ap, args)
-    if args.holdout < 0 or args.holdout >= len(poses):
-        ap.error(f"--holdout {args.holdout} must leave at least one of the {len(poses)} poses to train on")
-    try:
-        targets = read_targets(args.targets, len(poses), args.width, args.height)
-    except ValueError as e:
-        ap.error(str(e))
-    with np.load(args.input) as z:
-        d = {k: z[k] for k in z.files}
-    if "quant_map" in d or "quant_colors" in d:
-        ap.error(f"{args.input} is compressed: fine-tune the uncompressed tree first, then prune and compress")
-
-    from .host import Camera, RenderOptions
-    tree = load_tree_arrays(d, args.input)
-    opt = RenderOptions(step_size=args.step_size, sigma_thresh=args.sigma_thresh, stop_thresh=args.stop_thresh,
-                        background_brightness=args.background)
-    cams = []
-    for m in poses:
-        c = Camera(args.width, args.height, fx, fy)
-        c.set_c2w(m)
-        cams.append(c)
+    tree, cams, targets, d, opt = open_inputs(ap, args, _ADVICE, holdout=args.holdout)
     n_train = len(cams) - args.holdout
     held = list(range(n_train, len(cams)))
     if held:

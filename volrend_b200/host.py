@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import copy
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass, field
 
@@ -285,12 +286,8 @@ class N3Tree:
         never describes two different trees.  Asynchronous on ``stream``.  The tree must be loaded with
         ``load_cuda(slot_map=True)``."""
         import torch
-        if not self.is_cuda_loaded():
-            raise RuntimeError("N3Tree is not loaded on the device")
-        if not self._slot_map:
-            raise RuntimeError("update_data needs the slot map: load the tree with load_cuda(slot_map=True)")
+        dev = _slot_tree(self, "update_data")
         shape = (self.capacity, self.N, self.N, self.N, self.data_dim)
-        dev = torch.device("cuda", self._device)
         if (not isinstance(data, torch.Tensor) or data.dtype not in (torch.float16, torch.float32)
                 or data.device != dev or tuple(data.shape) != shape):
             raise ValueError(f"data must be a float16 or float32 tensor of shape {shape} on {dev}")
@@ -671,29 +668,13 @@ def leaf_weights(tree: N3Tree, cams, options: RenderOptions, out=None, alpha=Non
     device tensor, accumulated.  Asynchronous on ``stream``.  The tree must be loaded with
     ``load_cuda(slot_map=True)``."""
     import torch
-    if not tree.is_cuda_loaded():
-        raise RuntimeError("N3Tree is not loaded on the device")
-    if not tree._slot_map:
-        raise RuntimeError("leaf_weights needs the slot map: load the tree with load_cuda(slot_map=True)")
-    if isinstance(cams, Camera):
-        cams = [cams]
-    if not isinstance(options, RenderOptions):
-        raise TypeError("leaf_weights takes one RenderOptions for every view")
-    dev = torch.device("cuda", tree._device)
-    n_slots = tree.capacity * tree.N ** 3
-    if out is None:
-        out = torch.full((tree.capacity, tree.N, tree.N, tree.N), float("-inf"), dtype=torch.float32, device=dev)
-    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
-          or not out.is_contiguous() or out.numel() != n_slots):
-        raise ValueError(f"out must be a contiguous float32 tensor of {n_slots} elements on {dev}")
-    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if cams else (0, 0)
-    if alpha is not None and (alpha.dtype != torch.float32 or alpha.device != dev or not alpha.is_contiguous()
-                              or alpha.numel() != len(cams) * w * h):
-        raise ValueError(f"alpha must be a contiguous float32 tensor of {len(cams)} x {h} x {w} elements on {dev}")
-    arr = _cams_array(cams)
-    o = options._as_c()
-    check(lib().vr_tree_leaf_weights(tree._handle, arr, len(cams), C.byref(o), _rect(tile), out.data_ptr(),
-                                     alpha.data_ptr() if alpha is not None else None,
+    dev = _slot_tree(tree, "leaf_weights")
+    cams, w, h = _march_views(cams, options, tile, "leaf_weights")
+    out = _accumulator("out", out, (tree.capacity, tree.N, tree.N, tree.N), float("-inf"), torch.float32, dev)
+    if alpha is not None:
+        _check_tensor("alpha", alpha, torch.float32, len(cams) * w * h, dev)
+    check(lib().vr_tree_leaf_weights(tree._handle, _cams_array(cams), len(cams), C.byref(options._as_c()), _rect(tile),
+                                     out.data_ptr(), alpha.data_ptr() if alpha is not None else None,
                                      counters.data_ptr() if counters is not None else None, _stream_ptr(stream)))
     return out
 
@@ -708,29 +689,12 @@ def leaf_error(tree: N3Tree, cams, options: RenderOptions, err, out=None, counte
     tensor, accumulated.  Asynchronous on ``stream``; the sums are atomic, so they vary in the last bits from run to
     run.  The tree must be loaded with ``load_cuda(slot_map=True)``."""
     import torch
-    if not tree.is_cuda_loaded():
-        raise RuntimeError("N3Tree is not loaded on the device")
-    if not tree._slot_map:
-        raise RuntimeError("leaf_error needs the slot map: load the tree with load_cuda(slot_map=True)")
-    if isinstance(cams, Camera):
-        cams = [cams]
-    if not isinstance(options, RenderOptions):
-        raise TypeError("leaf_error takes one RenderOptions for every view")
-    dev = torch.device("cuda", tree._device)
-    n_slots = tree.capacity * tree.N ** 3
-    if out is None:
-        out = torch.zeros((tree.capacity, tree.N, tree.N, tree.N), dtype=torch.float32, device=dev)
-    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
-          or not out.is_contiguous() or out.numel() != n_slots):
-        raise ValueError(f"out must be a contiguous float32 tensor of {n_slots} elements on {dev}")
-    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if cams else (0, 0)
-    if (not isinstance(err, torch.Tensor) or err.dtype != torch.float32 or err.device != dev
-            or not err.is_contiguous() or err.numel() != len(cams) * w * h):
-        raise ValueError(f"err must be a contiguous float32 tensor of {len(cams)} x {h} x {w} elements on {dev}")
-    arr = _cams_array(cams)
-    o = options._as_c()
-    check(lib().vr_tree_leaf_error(tree._handle, arr, len(cams), C.byref(o), _rect(tile), err.data_ptr(),
-                                   out.data_ptr(), counters.data_ptr() if counters is not None else None,
+    dev = _slot_tree(tree, "leaf_error")
+    cams, w, h = _march_views(cams, options, tile, "leaf_error")
+    out = _accumulator("out", out, (tree.capacity, tree.N, tree.N, tree.N), 0.0, torch.float32, dev)
+    _check_tensor("err", err, torch.float32, len(cams) * w * h, dev)
+    check(lib().vr_tree_leaf_error(tree._handle, _cams_array(cams), len(cams), C.byref(options._as_c()), _rect(tile),
+                                   err.data_ptr(), out.data_ptr(), counters.data_ptr() if counters is not None else None,
                                    _stream_ptr(stream)))
     return out
 
@@ -745,45 +709,37 @@ def leaf_grads(tree: N3Tree, cams, options: RenderOptions, dpix, out=None, float
     are atomic, so they vary in the last bits from run to run.  The tree must be loaded with
     ``load_cuda(slot_map=True)``."""
     import torch
-    if not tree.is_cuda_loaded():
-        raise RuntimeError("N3Tree is not loaded on the device")
-    if not tree._slot_map:
-        raise RuntimeError("leaf_grads needs the slot map: load the tree with load_cuda(slot_map=True)")
-    if isinstance(cams, Camera):
-        cams = [cams]
-    if not isinstance(options, RenderOptions):
-        raise TypeError("leaf_grads takes one RenderOptions for every view")
-    dev = torch.device("cuda", tree._device)
-    n = tree.capacity * tree.N ** 3 * tree.data_dim
-    if out is None:
-        out = torch.zeros((tree.capacity, tree.N, tree.N, tree.N, tree.data_dim), dtype=torch.float32, device=dev)
-    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
-          or not out.is_contiguous() or out.numel() != n):
-        raise ValueError(f"out must be a contiguous float32 tensor of {n} elements on {dev}")
-    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if cams else (0, 0)
-    npx = len(cams) * w * h * 4
-    for name, t in (("dpix", dpix), ("float_out", float_out)):
-        if t is None and name == "float_out":
-            continue
-        if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous()
-                or t.numel() != npx):
-            raise ValueError(f"{name} must be a contiguous float32 tensor of {len(cams)} x {h} x {w} x 4 elements "
-                             f"on {dev}")
-    arr = _cams_array(cams)
-    o = options._as_c()
-    check(lib().vr_tree_leaf_grads(tree._handle, arr, len(cams), C.byref(o), _rect(tile), dpix.data_ptr(),
-                                   out.data_ptr(), float_out.data_ptr() if float_out is not None else None,
+    dev = _slot_tree(tree, "leaf_grads")
+    cams, w, h = _march_views(cams, options, tile, "leaf_grads")
+    out = _accumulator("out", out, (tree.capacity, tree.N, tree.N, tree.N, tree.data_dim), 0.0, torch.float32, dev)
+    _check_tensor("dpix", dpix, torch.float32, len(cams) * w * h * 4, dev)
+    if float_out is not None:
+        _check_tensor("float_out", float_out, torch.float32, len(cams) * w * h * 4, dev)
+    check(lib().vr_tree_leaf_grads(tree._handle, _cams_array(cams), len(cams), C.byref(options._as_c()), _rect(tile),
+                                   dpix.data_ptr(), out.data_ptr(), float_out.data_ptr() if float_out is not None else None,
                                    _stream_ptr(stream)))
     return out
 
 
-def _tv_tree(tree: N3Tree, what: str):
+def _slot_tree(tree: N3Tree, what: str):
+    """The CUDA device of ``tree``, which must be loaded with the slot map that ``what`` needs."""
     import torch
     if not tree.is_cuda_loaded():
         raise RuntimeError("N3Tree is not loaded on the device")
     if not tree._slot_map:
         raise RuntimeError(f"{what} needs the slot map: load the tree with load_cuda(slot_map=True)")
     return torch.device("cuda", tree._device)
+
+
+def _march_views(cams, options, tile, what: str):
+    """(cams, w, h) of a march-based leaf pass: the cameras as a list (one Camera: one view) and the size of the tile,
+    or of the views' frame, that the per-pixel tensors cover."""
+    if isinstance(cams, Camera):
+        cams = [cams]
+    if not isinstance(options, RenderOptions):
+        raise TypeError(f"{what} takes one RenderOptions for every view")
+    w, h = (int(tile[2]), int(tile[3])) if tile is not None else (cams[0].width, cams[0].height) if cams else (0, 0)
+    return cams, w, h
 
 
 def _check_tensor(name: str, t, dtype, n: int, dev) -> None:
@@ -794,6 +750,16 @@ def _check_tensor(name: str, t, dtype, n: int, dev) -> None:
                          f"on {dev}")
 
 
+def _accumulator(name: str, t, shape, fill: float, dtype, dev):
+    """A pass's accumulating output: ``t`` checked to hold as many ``dtype`` elements as ``shape`` on ``dev``, or
+    without it a new tensor of ``shape`` that starts at ``fill``."""
+    import torch
+    if t is None:
+        return torch.full(shape, fill, dtype=dtype, device=dev)
+    _check_tensor(name, t, dtype, math.prod(shape), dev)
+    return t
+
+
 def leaf_neighbors(tree: N3Tree, out=None, stream=None):
     """Forward neighbour of every leaf slot along x, y and z (vr_tree_leaf_neighbors): a CUDA int32 tensor
     ``[capacity * 8, 3]`` holding, for a reachable leaf slot at depth d with integer cell i, the slot of the leaf whose
@@ -802,7 +768,7 @@ def leaf_neighbors(tree: N3Tree, out=None, stream=None):
     ``stream`` (the first call for a tree counts its cells and synchronises it).  The tree must be loaded with
     ``load_cuda(slot_map=True)``; a structural change (a new ``load_cuda``) needs a new table."""
     import torch
-    dev = _tv_tree(tree, "leaf_neighbors")
+    dev = _slot_tree(tree, "leaf_neighbors")
     n = tree.capacity * tree.N ** 3
     if out is None:
         out = torch.empty((n, 3), dtype=torch.int32, device=dev)
@@ -822,22 +788,15 @@ def leaf_tv(tree: N3Tree, nbr, data, lambda_sigma: float, lambda_color: float, o
     >= 0; a weight of 0 skips its group.  Asynchronous on ``stream``; the gradient sums are atomic, so they vary in the
     last bits from run to run."""
     import torch
-    dev = _tv_tree(tree, "leaf_tv")
-    n_slots = tree.capacity * tree.N ** 3
-    n = n_slots * tree.data_dim
+    dev = _slot_tree(tree, "leaf_tv")
+    shape = (tree.capacity, tree.N, tree.N, tree.N, tree.data_dim)
     for name, w in (("lambda_sigma", lambda_sigma), ("lambda_color", lambda_color)):
         if not (float(w) >= 0.0) or float(w) == float("inf"):
             raise ValueError(f"{name} {w} must be finite and >= 0")
-    _check_tensor("nbr", nbr, torch.int32, n_slots * 3, dev)
-    _check_tensor("data", data, torch.float32, n, dev)
-    if out is None:
-        out = torch.zeros((tree.capacity, tree.N, tree.N, tree.N, tree.data_dim), dtype=torch.float32, device=dev)
-    else:
-        _check_tensor("out", out, torch.float32, n, dev)
-    if energy is None:
-        energy = torch.zeros(1, dtype=torch.float64, device=dev)
-    else:
-        _check_tensor("energy", energy, torch.float64, 1, dev)
+    _check_tensor("nbr", nbr, torch.int32, math.prod(shape[:4]) * 3, dev)
+    _check_tensor("data", data, torch.float32, math.prod(shape), dev)
+    out = _accumulator("out", out, shape, 0.0, torch.float32, dev)
+    energy = _accumulator("energy", energy, (1,), 0.0, torch.float64, dev)
     check(lib().vr_tree_leaf_tv(tree._handle, nbr.data_ptr(), data.data_ptr(), float(lambda_sigma),
                                 float(lambda_color), out.data_ptr(), energy.data_ptr(), _stream_ptr(stream)))
     return out, energy

@@ -21,14 +21,15 @@ from __future__ import annotations
 
 import argparse
 import math
-import os
 import sys
 
 import numpy as np
 
-from .compress import DROPPED_KEYS, _write_npz
+from .compress import _write_npz, carried_keys, check_uncompressed
+from .views import add_view_arguments, open_inputs
 
 N = 2
+_ADVICE = "prune the uncompressed tree first, then compress"
 
 
 def _structure(child: np.ndarray):
@@ -118,86 +119,15 @@ def prune_npz(z, weights, thresh: float, collapse: bool = True) -> dict:
     """The pruned form of the tree dict ``z`` (``N3Tree`` npz keys): ``child`` and ``data`` pruned by
     :func:`prune_arrays`, the training-time keys ``compress_npz`` drops dropped too, every other key passed through.
     Compressed input (``quant_map``) is refused: prune first, then compress."""
-    keys = list(z.files if hasattr(z, "files") else z)
-    if "quant_map" in keys or "quant_colors" in keys:
-        raise ValueError("the tree is already compressed (quant_map): prune the uncompressed tree first, then compress")
-    for k in ("child", "data"):
-        if k not in keys:
-            raise ValueError(f"the tree has no '{k}' array")
+    check_uncompressed(z, _ADVICE)
     child, data = prune_arrays(z["child"], z["data"], weights, thresh, collapse)
-    out = {k: z[k] for k in keys if k not in ("child", "data") and k not in DROPPED_KEYS}
+    out = {k: z[k] for k in carried_keys(z, ("child", "data"))}
     out["child"] = child
     out["data"] = data
     return out
 
 
 # ---------------------------------------------------------------------------------------------------------- CLI
-def read_poses(path: str) -> list:
-    """Row-major 4x4 camera-to-world matrices of a pose file, one or more per file (volrend_headless)."""
-    with open(path) as f:
-        vals = np.array(f.read().split(), np.float32)
-    n = vals.size // 16 + (1 if vals.size % 16 >= 12 else 0)
-    vals = np.concatenate([vals, np.zeros(n * 16 - vals.size, np.float32)]) if n * 16 > vals.size else vals
-    return [vals[16 * i:16 * i + 16].reshape(4, 4) for i in range(n)]
-
-
-def read_intrinsics(path: str):
-    """(fx, fy) of a 4x4 intrinsics file: the first and the sixth number (volrend_headless)."""
-    with open(path) as f:
-        vals = f.read().split()
-    if len(vals) < 6:
-        raise ValueError(f"intrinsics file {path} has {len(vals)} numbers, not a 4x4 matrix")
-    return float(vals[0]), float(vals[5])
-
-
-def add_view_arguments(ap: argparse.ArgumentParser) -> None:
-    """The camera, pose and march options of the tools that run views over a tree (prune, finetune):
-    volrend_headless's pose files, -i, -r and image size, and the step and thresholds."""
-    ap.add_argument("poses", nargs="+", help="camera-to-world pose .txt files (row-major 4x4, one or more per file)")
-    ap.add_argument("-i", "--intrin", default="", help="intrinsics matrix 4x4; if set, overrides the fx/fy")
-    ap.add_argument("-r", "--reverse_yz", action="store_true", help="use OpenCV camera space convention instead of NeRF")
-    ap.add_argument("--width", type=int, default=800, help="image width")
-    ap.add_argument("--height", type=int, default=800, help="image height")
-    ap.add_argument("--fx", type=float, default=-1.0, help="focal length in x (default 1111.11)")
-    ap.add_argument("--fy", type=float, default=-1.0, help="focal length in y (default fx)")
-    ap.add_argument("--step_size", type=float, default=1e-4, help="ray march step size")
-    ap.add_argument("--sigma_thresh", type=float, default=1e-2, help="sigma threshold of a shaded sample")
-    ap.add_argument("--stop_thresh", type=float, default=1e-2, help="transmittance below which a ray stops")
-
-
-def view_setup(ap: argparse.ArgumentParser, args):
-    """Checks add_view_arguments' values (ap.error on a bad one) -> (row-major 4x4 poses, fx, fy)."""
-    if args.width < 1 or args.height < 1:
-        ap.error(f"image size {args.width}x{args.height} must be positive")
-    for p in args.poses + ([args.intrin] if args.intrin else []):
-        if not os.path.exists(p):
-            ap.error(f"'{p}' does not exist")
-    fx = 1111.11 if args.fx < 0 else args.fx
-    fy = fx if args.fy < 0 else args.fy
-    if args.intrin:
-        fx, fy = read_intrinsics(args.intrin)
-    poses = [m for p in args.poses for m in read_poses(p)]
-    if not poses:
-        ap.error("no camera poses in the pose files")
-    if args.reverse_yz:
-        poses = [m @ np.diag([1, -1, -1, 1]).astype(np.float32) for m in poses]
-    return poses, fx, fy
-
-
-def load_tree_arrays(d: dict, path: str):
-    """An N3Tree of the npz dict ``d`` read from ``path``, on the device with the slot map; NDC trees (a
-    ``<tree>_poses_bounds.npy`` beside the file) as ``N3Tree.open`` loads them."""
-    from .host import N3Tree
-    tree = N3Tree()
-    tree.load_npz(d)
-    pb = path[:-4] + "_poses_bounds.npy"
-    if path.endswith(".npz") and os.path.exists(pb):
-        tree.use_ndc = True
-        tree._unpack_llff_poses_bounds(np.load(pb))
-    tree.load_cuda(slot_map=True)
-    return tree
-
-
 def _parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(prog="python -m volrend_b200.prune",
                                  description="Prune a PlenOctree npz by ray weight: leaves whose maximum compositing "
@@ -215,30 +145,13 @@ def _parser() -> argparse.ArgumentParser:
 def main(argv=None) -> int:
     ap = _parser()
     args = ap.parse_args(argv)
-    if args.width < 1 or args.height < 1:
-        ap.error(f"image size {args.width}x{args.height} must be positive")
     if math.isnan(args.thresh):
         ap.error("--thresh is NaN")
     if args.batch < 1:
         ap.error(f"--batch {args.batch} < 1")
-    if os.path.abspath(args.input) == os.path.abspath(args.output):
-        ap.error("the output would overwrite the input")
-    if not os.path.exists(args.input):
-        ap.error(f"'{args.input}' does not exist")
-    poses, fx, fy = view_setup(ap, args)
-    with np.load(args.input) as z:
-        d = {k: z[k] for k in z.files}
-    if "quant_map" in d or "quant_colors" in d:
-        ap.error(f"{args.input} is already compressed: prune the uncompressed tree first, then compress")
+    tree, cams, _, d, opt = open_inputs(ap, args, _ADVICE)
 
-    from .host import Camera, RenderOptions, leaf_weights
-    tree = load_tree_arrays(d, args.input)
-    opt = RenderOptions(step_size=args.step_size, sigma_thresh=args.sigma_thresh, stop_thresh=args.stop_thresh)
-    cams = []
-    for m in poses:
-        c = Camera(args.width, args.height, fx, fy)
-        c.set_c2w(m)
-        cams.append(c)
+    from .host import leaf_weights
     w = None
     for v0 in range(0, len(cams), args.batch):
         w = leaf_weights(tree, cams[v0:v0 + args.batch], opt, out=w)

@@ -24,16 +24,17 @@ from __future__ import annotations
 
 import argparse
 import math
-import os
 import sys
 
 import numpy as np
 
-from .compress import DROPPED_KEYS, _write_npz
-from .prune import N, _structure, add_view_arguments, load_tree_arrays, view_setup
+from .compress import _write_npz, carried_keys, check_uncompressed
+from .prune import N, _structure
+from .views import add_view_arguments, open_inputs, pixel_error, target_batch
 
 MAX_TREE_DEPTH = 23            # kMaxTreeDepth: the deepest leaf level vr_tree_create accepts
 MAX_NODES = 0xFFFFFFFF // 8    # the slot map holds node * 8 + octant in a u32 with 0xffffffff reserved
+_ADVICE = "refine the uncompressed tree first, then prune and compress"
 
 
 def check_capacity(n_nodes: int) -> None:
@@ -85,27 +86,16 @@ def refine_npz(z, scores, fraction: float, max_depth: int = MAX_TREE_DEPTH) -> d
     gathered by its ``src`` in the source's dtype, the training-time keys ``compress_npz`` drops dropped, every other
     key (``extra_data`` included) passed through.  Compressed input (``quant_map``) is refused: refine and fit first,
     then prune and compress."""
-    keys = list(z.files if hasattr(z, "files") else z)
-    if "quant_map" in keys or "quant_colors" in keys:
-        raise ValueError("the tree is compressed (quant_map): refine the uncompressed tree, then prune and compress")
-    for k in ("child", "data"):
-        if k not in keys:
-            raise ValueError(f"the tree has no '{k}' array")
+    check_uncompressed(z, _ADVICE)
     data = np.asarray(z["data"])
     if data.ndim != 5 or data.shape[:4] != np.asarray(z["child"]).shape:
         raise ValueError(f"data has shape {data.shape}, not [capacity, 2, 2, 2, data_dim]")
     child, src = refine_plan(z["child"], scores, fraction, max_depth)
     dd = data.shape[-1]
-    out = {k: z[k] for k in keys if k not in ("child", "data") and k not in DROPPED_KEYS}
+    out = {k: z[k] for k in carried_keys(z, ("child", "data"))}
     out["child"] = child
     out["data"] = data.reshape(-1, dd)[src].reshape(-1, N, N, N, dd)
     return out
-
-
-def pixel_error(render, target):
-    """The pixel error the CLIs and the coarse-to-fine fit score leaves with: the squared RGB error of a float render
-    ``[..., 4]`` against background-composited RGB targets ``[..., 3]``, summed over the channels."""
-    return (render[..., :3] - target).square().sum(-1)
 
 
 def leaf_scores(tree, cams, targets, options, batch: int, out=None):
@@ -113,7 +103,6 @@ def leaf_scores(tree, cams, targets, options, batch: int, out=None):
     rendered and scored in batches of ``batch`` views: a float32 CUDA tensor [capacity, 2, 2, 2], accumulated into
     ``out`` when given."""
     import torch
-    from .finetune import _target_rgb
     from .host import leaf_error, render_batch
     dev = torch.device("cuda", tree._device)
     H, W = cams[0].height, cams[0].width
@@ -121,10 +110,7 @@ def leaf_scores(tree, cams, targets, options, batch: int, out=None):
         vc = cams[v0:v0 + batch]
         fo = torch.empty((len(vc), H, W, 4), dtype=torch.float32, device=dev)
         render_batch(tree, vc, options, None, float_out=fo)
-        tgt = torch.stack([_target_rgb(targets[v], options.background_brightness, dev)
-                           for v in range(v0, v0 + len(vc))])
-        if tuple(tgt.shape) != (len(vc), H, W, 3):
-            raise ValueError(f"targets are {tuple(tgt.shape[1:3])}, the views {H}x{W}")
+        tgt = target_batch(targets, range(v0, v0 + len(vc)), options.background_brightness, dev, H, W)
         out = leaf_error(tree, vc, options, pixel_error(fo, tgt).contiguous(), out=out)
     return out
 
@@ -137,11 +123,7 @@ def _parser() -> argparse.ArgumentParser:
                                              "error, summed on the GPU).")
     ap.add_argument("input", help="npz file storing octree data (uncompressed)")
     ap.add_argument("output", help="where to write the refined npz")
-    add_view_arguments(ap)
-    ap.add_argument("--targets", nargs="+", required=True,
-                    help="one PNG per pose, or one .npy [views, height, width, 3|4] (uint8 or float in [0, 1])")
-    ap.add_argument("--background", type=float, default=1.0,
-                    help="background brightness: renders and the compositing of RGBA targets")
+    add_view_arguments(ap, targets=True)
     ap.add_argument("--fraction", type=float, required=True,
                     help="share of the candidate leaves (positive score, above --max-depth) to split, in [0, 1]")
     ap.add_argument("--max-depth", type=int, default=MAX_TREE_DEPTH,
@@ -151,7 +133,6 @@ def _parser() -> argparse.ArgumentParser:
 
 
 def main(argv=None) -> int:
-    from .finetune import read_targets
     ap = _parser()
     args = ap.parse_args(argv)
     if not (0.0 <= args.fraction <= 1.0):
@@ -160,30 +141,7 @@ def main(argv=None) -> int:
         ap.error(f"--max-depth {args.max_depth} < 1")
     if args.batch < 1:
         ap.error(f"--batch {args.batch} < 1")
-    if os.path.abspath(args.input) == os.path.abspath(args.output):
-        ap.error("the output would overwrite the input")
-    for p in [args.input] + args.targets:
-        if not os.path.exists(p):
-            ap.error(f"'{p}' does not exist")
-    poses, fx, fy = view_setup(ap, args)
-    try:
-        targets = read_targets(args.targets, len(poses), args.width, args.height)
-    except ValueError as e:
-        ap.error(str(e))
-    with np.load(args.input) as z:
-        d = {k: z[k] for k in z.files}
-    if "quant_map" in d or "quant_colors" in d:
-        ap.error(f"{args.input} is compressed: refine the uncompressed tree first, then prune and compress")
-
-    from .host import Camera, RenderOptions
-    tree = load_tree_arrays(d, args.input)
-    opt = RenderOptions(step_size=args.step_size, sigma_thresh=args.sigma_thresh, stop_thresh=args.stop_thresh,
-                        background_brightness=args.background)
-    cams = []
-    for m in poses:
-        c = Camera(args.width, args.height, fx, fy)
-        c.set_c2w(m)
-        cams.append(c)
+    tree, cams, targets, d, opt = open_inputs(ap, args, _ADVICE)
     scores = leaf_scores(tree, cams, targets, opt, args.batch).cpu().numpy().reshape(-1)
     tree.free_cuda()
     out = refine_npz(d, scores, args.fraction, args.max_depth)
