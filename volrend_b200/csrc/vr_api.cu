@@ -195,6 +195,11 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
     {
         std::lock_guard<std::mutex> lk(mt->res_mu);
         cfg.work_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(sr->queues) + (size_t)(sr->next_queue++ % kQueueSlots) * kQueueSlotBytes);
+        // The kernels read the tree before griddepcontrol.wait, and only that wait makes the predecessor's writes
+        // visible.  So the first launch on a stream after vr_tree_update_data rewrote the tree waits for its
+        // predecessor in full; later launches overlap again (the tree is not written between them).
+        cfg.pdl = sr->data_gen == mt->data_gen;
+        sr->data_gen = mt->data_gen;
     }
     // march_kernel above has rejected every kbd without kernels
     const cudaError_t e = pass == Pass::kWeights ? launch_weights(P, cfg) : pass == Pass::kError ? launch_error(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {

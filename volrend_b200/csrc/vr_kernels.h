@@ -33,6 +33,7 @@ struct LaunchCfg {
     bool queue;      // the shading-queue kernel, else the inline-shading one (march_kernel)
     bool count;      // instrumented build: accumulate vr_counters
     bool surface;    // write a cudaSurfaceObject instead of linear memory
+    bool pdl;        // launch with programmatic stream serialization (dispatch: not the first launch after an update)
     int num_sms;
     unsigned int* work_counter;  // persistent kernels: {work head, done CTAs}
     cudaStream_t stream;

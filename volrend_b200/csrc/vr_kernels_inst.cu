@@ -90,7 +90,7 @@ cudaError_t launch_persistent_grid(K kernel, size_t smem, LaunchDev& P, const La
     cudaLaunchAttribute attr[1];   // programmatic dependent launch: see pdl_wait_predecessor() in vr_march.cuh
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    lc.attrs = attr; lc.numAttrs = 1;
+    lc.attrs = attr; lc.numAttrs = cfg.pdl ? 1 : 0;
     return cudaLaunchKernelEx(&lc, kernel, P);
 }
 

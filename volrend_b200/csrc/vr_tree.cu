@@ -492,6 +492,10 @@ int vr_tree_update_data(vr_tree* t, const uint16_t* data_dev, void* stream) {
                                                                                             n_entries, rec_bytes, t->wide);
     VR_CUDA(cudaGetLastError());
     g_launches += 1;
+    {
+        std::lock_guard<std::mutex> lk(t->res_mu);
+        ++t->data_gen;
+    }
     return VR_OK;
 }
 

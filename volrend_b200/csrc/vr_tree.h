@@ -54,6 +54,7 @@ struct StreamRes {
     vrb::OptDev* opt_ring = nullptr; // kCamRing entries beside cam_ring (same slots), allocated by the first
                                      // batch with options per view
     unsigned int next_queue = 0, cam_pos = 0;
+    unsigned long long data_gen = 0; // the tree's data_gen at this stream's last march launch
 };
 
 struct vr_tree {
@@ -70,6 +71,9 @@ struct vr_tree {
     long long n_tables = 0;
     std::mutex res_mu;
     std::unordered_map<cudaStream_t, StreamRes> res;
+    // bumped (under res_mu) by every vr_tree_update_data: a stream's first march launch after an update is made
+    // without programmatic dependent launch, since the march reads the tree before griddepcontrol.wait (dispatch)
+    unsigned long long data_gen = 0;
     // vr_render_frames_host: chunk ring, streams and events are created once and kept
     struct HostPath {
         static constexpr int kRing = 4;
