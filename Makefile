@@ -42,6 +42,10 @@ $(OBJ)/vr_tree.o: volrend_b200/csrc/vr_tree.cu volrend_b200/csrc/vr_tree.h volre
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_tree.log || (cat $(OBJ)/ptxas_tree.log; false)
 
+$(OBJ)/vr_cull.o: volrend_b200/csrc/vr_cull.cu volrend_b200/csrc/vr_tree.h volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_wire.h include/volrend_b200.h
+	@mkdir -p $(OBJ)
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_cull.log || (cat $(OBJ)/ptxas_cull.log; false)
+
 $(OBJ)/vr_raster.o: volrend_b200/csrc/vr_raster.cu volrend_b200/csrc/vr_raster.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_raster.log || (cat $(OBJ)/ptxas_raster.log; false)
@@ -78,7 +82,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp volrend_b200/csrc/vr_frames.h incl
 	@mkdir -p $(OBJ)
 	$(CXX) -O3 -std=c++17 -fPIC -Iinclude -c $< -o $@
 
-$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_tv.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
+$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_cull.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_tv.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
 oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/liberror_oracle.so oracle/libsurface_harness.so

@@ -107,8 +107,9 @@ typedef struct {
                                         the v with fewer tables is chosen per tree */
     int64_t n_tables;
     int64_t wide_bytes, wrecs_bytes; /* 64-entry tables; colour records indexed by table entry */
-    int64_t kernel_bytes;            /* what the march kernels can touch: wide_bytes + wrecs_bytes */
+    int64_t kernel_bytes;            /* what the render kernels can touch: wide_bytes + wrecs_bytes + grid_bytes */
     int64_t device_bytes;            /* everything the tree keeps resident */
+    int64_t grid_bytes;              /* coarse max-sigma grid (32^3 cells) that batch renders cull ray tiles with */
 } vr_tree_info;
 
 /* Compressed N3Tree as written by scripts/compress_octree.py:93-118 (keys quant_colors, quant_map,
@@ -379,7 +380,9 @@ int vr_mg_render(vr_mg* mg, const vr_camera* cams, int n_views, const vr_options
                  uint8_t* rgba8_dev0, uint8_t* rgba8_host, float* ms_out);
 const uint8_t* vr_mg_frames_dev0(const vr_mg* mg);
 const char* vr_mg_last_error(const vr_mg* mg);
-/* How many of this library's kernels were launched by this process. */
+/* How many of this library's kernels were launched by this process.  One exception: a batch render's tile-coverage
+ * pass (the kernel that decides which ray tiles of the batch can shade) is not counted on its own but with the march
+ * launch it prepares, so a batch march still counts as one launch. */
 unsigned long long vr_launch_count(void);
 
 const char* vr_last_error(void);

@@ -6,6 +6,9 @@
  *   P0  one 4x8 tile per warp pass, inline shading (the round-1 kernel)
  *   P1  P0 + warp-shared shading queue drained 32 items at a time
  *   P2  ray-granular refill from a per-warp pool of set-up rays (threshold = idle lanes) + P1 queue
+ *   CULL=1  instead: the tile culling of batch launches (vr_cull.cu) -- tiles and warp instructions it culls, next
+ *           to the bound of culling every tile where no ray shades, and a check that no tile with a shading ray
+ *           is culled (exit code 1 if one is); THRESH=<sigma_thresh> overrides the default threshold
  *
  * Cost constants (warp instructions) come from the SASS of the round-1 kernel.
  * Usage: lane_sim <dump.bin> ; the dump is written by tools/lane_sim.py.
@@ -672,6 +675,161 @@ static void mem_main(const orc_tree* tree, const orc_camera* cams, int ncam, int
     }
 }
 
+/* ---- tile culling of batch launches: the policy of volrend_b200/csrc/vr_cull.cu restated on the CPU, with the
+   same grid level (32^3 cells of the largest sigma of the reachable leaves), the same dilation (eps in tree space,
+   dpx in pixels) and the same granularity (one bit per 4x8 tile).  No NDC trees, no bands, no render_bbox other than
+   the unit cube here: the kernel marks whole views for those. */
+#define CULL_LV 5
+#define CULL_N (1 << CULL_LV)
+#define CULL_CELL_TILES_MAX 1024   /* kCellTilesMax: a larger cell marks the whole view */
+static float g_cgrid[CULL_N * CULL_N * CULL_N];
+static float g_csmin;
+
+static void cull_visit(const orc_tree* tree, int64_t node, int depth, uint32_t ox, uint32_t oy, uint32_t oz) {
+    const int sh = 23 - depth;   /* children of a node of depth `depth` have cubes of 2^(24 - depth - 1) units */
+    for (int oct = 0; oct < 8; ++oct) {
+        const uint32_t x = ox | ((uint32_t)(oct >> 2 & 1) << sh), y = oy | ((uint32_t)(oct >> 1 & 1) << sh),
+                       z = oz | ((uint32_t)(oct & 1) << sh);
+        const int64_t s = node * 8 + oct;
+        const int32_t skip = tree->child[s];
+        if (skip) { cull_visit(tree, node + skip, depth + 1, x, y, z); continue; }
+        const float sg = h2f(tree->data[(size_t)s * tree->data_dim + tree->data_dim - 1]);
+        if (sg != sg) continue;
+        if (sg < g_csmin) g_csmin = sg;
+        const int cs = 24 - CULL_LV;
+        const uint32_t span = (1u << sh) - 1u;
+        for (uint32_t cx = x >> cs; cx <= (x + span) >> cs; ++cx)
+            for (uint32_t cy = y >> cs; cy <= (y + span) >> cs; ++cy)
+                for (uint32_t cz = z >> cs; cz <= (z + span) >> cs; ++cz) {
+                    float* c = &g_cgrid[(cx * CULL_N + cy) * CULL_N + cz];
+                    if (sg > *c) *c = sg;
+                }
+    }
+}
+
+static void cull_grid(const orc_tree* tree) {
+    for (int i = 0; i < CULL_N * CULL_N * CULL_N; ++i) g_cgrid[i] = -INFINITY;
+    g_csmin = INFINITY;
+    cull_visit(tree, 0, 0, 0, 0, 0);
+}
+
+/* mask[ty * tiles_x + tx] = 1: the tile may hold a ray that shades (vr_cull.cu tile_mask_kernel) */
+static void cull_mask(const orc_tree* tree, const orc_camera* cam, const orc_options* opt, uint8_t* mask) {
+    const int W = cam->width, H = cam->height, ntx = (W + 3) / 4, nty = (H + 7) / 8;
+    memset(mask, 0, (size_t)ntx * nty);
+    const float* c2w = cam->c2w;
+    const double M[9] = {c2w[0], c2w[3], -(double)c2w[6], c2w[1], c2w[4], -(double)c2w[7], c2w[2], c2w[5], -(double)c2w[8]};
+    const double a0 = M[4] * M[8] - M[5] * M[7], a1 = M[5] * M[6] - M[3] * M[8], a2 = M[3] * M[7] - M[4] * M[6];
+    const double det = M[0] * a0 + M[1] * a1 + M[2] * a2;
+    int all = tree->ndc_width > 0.f || opt->sigma_thresh < g_csmin || !(fabs(det) > 0.0);
+    for (int i = 0; i < 3; ++i) all |= !(opt->render_bbox[i] >= 0.f && opt->render_bbox[i + 3] <= 1.f);
+    double m[9] = {0}, c[3] = {0}, l1 = 0.0;
+    if (!all) {
+        const double id = 1.0 / det;
+        m[0] = a0 * id; m[1] = (M[2] * M[7] - M[1] * M[8]) * id; m[2] = (M[1] * M[5] - M[2] * M[4]) * id;
+        m[3] = a1 * id; m[4] = (M[0] * M[8] - M[2] * M[6]) * id; m[5] = (M[2] * M[3] - M[0] * M[5]) * id;
+        m[6] = a2 * id; m[7] = (M[1] * M[6] - M[0] * M[7]) * id; m[8] = (M[0] * M[4] - M[1] * M[3]) * id;
+        for (int i = 0; i < 3; ++i) { c[i] = c2w[9 + i]; l1 += fabs((double)tree->scale[i] * c2w[9 + i] + tree->offset[i]); }
+    }
+    const double eps = 1e-5 * (4.0 + l1), sdpx = 1e-5 * (fabs((double)cam->fx) + fabs((double)cam->fy));
+    for (int cell = 0; !all && cell < CULL_N * CULL_N * CULL_N; ++cell) {
+        if (!(g_cgrid[cell] > opt->sigma_thresh)) continue;
+        const int ci[3] = {cell >> (2 * CULL_LV), (cell >> CULL_LV) & (CULL_N - 1), cell & (CULL_N - 1)};
+        double lo[3], hi[3];
+        for (int i = 0; i < 3; ++i) {
+            const double a = ((double)ci[i] / CULL_N - eps - tree->offset[i]) / tree->scale[i];
+            const double b = ((double)(ci[i] + 1) / CULL_N + eps - tree->offset[i]) / tree->scale[i];
+            lo[i] = fmin(a, b) - c[i]; hi[i] = fmax(a, b) - c[i];
+        }
+        double wmin = INFINITY, wmax = -INFINITY, xmin = INFINITY, xmax = -INFINITY, ymin = INFINITY, ymax = -INFINITY,
+               vmax = 0.0;
+        for (int k = 0; k < 8; ++k) {
+            const double q0 = (k & 4) ? hi[0] : lo[0], q1 = (k & 2) ? hi[1] : lo[1], q2 = (k & 1) ? hi[2] : lo[2];
+            const double u = m[0] * q0 + m[1] * q1 + m[2] * q2, v = m[3] * q0 + m[4] * q1 + m[5] * q2,
+                         w = m[6] * q0 + m[7] * q1 + m[8] * q2;
+            wmin = fmin(wmin, w); wmax = fmax(wmax, w);
+            const double vx = u / w, vy = v / w;
+            vmax = fmax(vmax, fabs(vx) + fabs(vy));
+            const double px = vx * cam->fx + 0.5 * W, py = 0.5 * H - vy * cam->fy;
+            xmin = fmin(xmin, px); xmax = fmax(xmax, px); ymin = fmin(ymin, py); ymax = fmax(ymax, py);
+        }
+        if (wmax < 0.0) continue;
+        if (!(wmin > 0.0)) { all = 1; break; }
+        const double d = 1.0 + sdpx * (1.0 + vmax) * (1.0 + vmax);
+        const double fx0 = ceil(xmin - d), fx1 = floor(xmax + d), fy0 = ceil(ymin - d), fy1 = floor(ymax + d);
+        if (!(isfinite(fx0) && isfinite(fx1) && isfinite(fy0) && isfinite(fy1))) { all = 1; break; }
+        if (fx1 < 0 || fx0 > W - 1 || fy1 < 0 || fy0 > H - 1) continue;
+        const int tx0 = (int)fmax(fx0, 0.0) / 4, tx1 = (int)fmin(fx1, W - 1.0) / 4;
+        const int ty0 = (int)fmax(fy0, 0.0) / 8, ty1 = (int)fmin(fy1, H - 1.0) / 8;
+        if ((long long)(ty1 - ty0 + 1) * (tx1 - tx0 + 1) > CULL_CELL_TILES_MAX) { all = 1; break; }
+        for (int ty = ty0; ty <= ty1; ++ty)
+            for (int tx = tx0; tx <= tx1; ++tx) mask[ty * ntx + tx] = 1;
+    }
+    if (all) memset(mask, 1, (size_t)ntx * nty);
+}
+
+/* --cull: per view, the tiles the policy leaves unmarked although a ray in them shades (must be none), the tiles it
+   marks that never shade, and the share of warp body iterations and of warp instructions (cost model P0) it culls
+   next to the bound of culling exactly the tiles where no ray shades. */
+static int cull_main(const orc_tree* tree, const orc_camera* cams, int ncam, const orc_options* opt) {
+    const int W = cams[0].width, H = cams[0].height, ntx = (W + 3) / 4, nty = (H + 7) / 8;
+    ray_t* rays = (ray_t*)malloc((size_t)W * H * sizeof(ray_t));
+    uint8_t* mask = (uint8_t*)malloc((size_t)ntx * nty);
+    cull_grid(tree);
+    double T[7] = {0};   /* tiles, marked, shading, marked never shading, body, body culled, body bound */
+    stats_t sf = {0}, sc = {0}, sb = {0};
+    long long bad = 0;
+    for (int v = 0; v < ncam; ++v) {
+        g_trace_n = 0;
+        for (int y = 0; y < H; ++y)
+            for (int x = 0; x < W; ++x) trace_one(tree, &cams[v], opt, x, y, &rays[(size_t)y * W + x]);
+        cull_mask(tree, &cams[v], opt, mask);
+        long long vt[4] = {0, 0, 0, 0}, vbad = 0;
+        ray_t* cut = (ray_t*)malloc((size_t)W * H * sizeof(ray_t));
+        ray_t* ideal = (ray_t*)malloc((size_t)W * H * sizeof(ray_t));
+        memcpy(cut, rays, (size_t)W * H * sizeof(ray_t));
+        memcpy(ideal, rays, (size_t)W * H * sizeof(ray_t));
+        for (int ty = 0; ty < nty; ++ty)
+            for (int tx = 0; tx < ntx; ++tx) {
+                int shades = 0;
+                uint32_t body = 0;
+                for (int l = 0; l < 32; ++l) {
+                    const int x = tx * 4 + l % 4, y = ty * 8 + l / 4;
+                    if (x >= W || y >= H) continue;
+                    const ray_t* r = &rays[(size_t)y * W + x];
+                    if (r->n > body) body = r->n;
+                    for (uint32_t k = 0; k < r->n && !shades; ++k) shades = g_trace[r->off + k] >> 7;
+                }
+                const int mk = mask[ty * ntx + tx];
+                vt[0] += 1; vt[1] += mk; vt[2] += shades; vt[3] += mk && !shades;
+                if (shades && !mk) ++vbad;
+                T[4] += body; T[5] += mk ? 0 : body; T[6] += shades ? 0 : body;
+                for (int l = 0; l < 32; ++l) {
+                    const int x = tx * 4 + l % 4, y = ty * 8 + l / 4;
+                    if (x >= W || y >= H) continue;
+                    if (!mk) cut[(size_t)y * W + x].n = 0;
+                    if (!shades) ideal[(size_t)y * W + x].n = 0;
+                }
+            }
+        sim_tiles(rays, W, H, 0, &sf);
+        sim_tiles(cut, W, H, 0, &sc);
+        sim_tiles(ideal, W, H, 0, &sb);
+        free(cut); free(ideal);
+        printf("cull view %d: tiles %lld marked %lld shading %lld unmarked_shading %lld marked_never_shading %lld\n", v,
+               vt[0], vt[1], vt[2], vbad, vt[3]);
+        for (int k = 0; k < 4; ++k) T[k] += vt[k];
+        bad += vbad;
+    }
+    /* a culled tile skips its ray set-up too (C_SETUP of every tile in sim_tiles) */
+    const double setup_c = C_SETUP * (T[0] - T[1]), setup_b = C_SETUP * (T[0] - T[2]);
+    printf("cull total: views %d tiles %.0f unmarked_shading %lld tiles_culled %.4f (bound %.4f) marked_never_shading "
+           "%.4f body_culled %.4f (bound %.4f) instr_culled %.4f (bound %.4f)\n", ncam, T[0], bad, 1 - T[1] / T[0],
+           1 - T[2] / T[0], T[3] / T[0], T[5] / T[4], T[6] / T[4], 1 - (sc.instr - setup_c) / sf.instr,
+           1 - (sb.instr - setup_b) / sf.instr);
+    free(rays); free(mask);
+    return bad ? 1 : 0;
+}
+
 static void report(const char* name, const stats_t* S, int frames) {
     printf("%-34s %7.2f Minstr/frame  body %5.1f/32 (%6.2fM it)  fetch+ %5.1f/32 (%5.2fM)  shade %5.1f/32 (%5.3fM it)\n", name,
            S->instr / frames / 1e6, S->body_lanes / (S->body_iters + 1e-9), S->body_iters / frames / 1e6,
@@ -717,6 +875,15 @@ int main(int argc, char** argv) {
     for (int i = 0; i < 3; ++i) { tree.offset[i] = meta[i]; tree.scale[i] = meta[3 + i]; }
     orc_options opt;
     orc_default_options(&opt);
+    if (getenv("THRESH")) opt.sigma_thresh = (float)atof(getenv("THRESH"));
+    if (getenv("CULL") && atoi(getenv("CULL"))) {   /* tile culling of batch launches instead of the lane policies */
+        orc_camera* oc = (orc_camera*)calloc(ncam, sizeof(orc_camera));
+        for (int c = 0; c < ncam; ++c) {
+            oc[c].width = W; oc[c].height = H; oc[c].fx = meta[6]; oc[c].fy = meta[7];
+            memcpy(oc[c].c2w, cams + 12 * c, 48);
+        }
+        return cull_main(&tree, oc, ncam, &opt);
+    }
     if (getenv("MEM") && atoi(getenv("MEM"))) {   /* L2 replay of the work orders instead of the lane policies */
         g_mem = 1;
         orc_camera* oc = (orc_camera*)calloc(ncam, sizeof(orc_camera));

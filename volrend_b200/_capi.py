@@ -56,7 +56,7 @@ class vr_tree_info(C.Structure):
                 ("node_bytes", C.c_int64), ("rec_total_bytes", C.c_int64), ("top_bytes", C.c_int64),
                 ("kernel_basis", C.c_int32), ("wide_parity", C.c_int32), ("n_tables", C.c_int64),
                 ("wide_bytes", C.c_int64), ("wrecs_bytes", C.c_int64), ("kernel_bytes", C.c_int64),
-                ("device_bytes", C.c_int64)]
+                ("device_bytes", C.c_int64), ("grid_bytes", C.c_int64)]
 
 
 class vr_mesh_desc(C.Structure):

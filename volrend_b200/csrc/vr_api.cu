@@ -201,6 +201,10 @@ int dispatch(const vr_tree* t, LaunchDev& P, bool count, bool surface, cudaStrea
         cfg.pdl = sr->data_gen == mt->data_gen;
         sr->data_gen = mt->data_gen;
     }
+    // Batches on the inline kernel march only the tiles the coverage pass marks (vr_cull.cu); the instrumented
+    // kernels march every ray, so they need no mask.
+    if (pass == Pass::kRender && !count && kernel == MarchKernel::kInline && P.cams)
+        if (int rc = launch_tile_mask(mt, P, stream)) return rc;
     // march_kernel above has rejected every kbd without kernels
     const cudaError_t e = pass == Pass::kWeights ? launch_weights(P, cfg) : pass == Pass::kError ? launch_error(P, cfg) : with_kbd(t->dev.kbd, cudaErrorInvalidValue, [&](auto k) {
         return pass == Pass::kGrads ? launch_grads<decltype(k)::value>(P, cfg) : launch_march<decltype(k)::value>(P, cfg);

@@ -259,8 +259,10 @@ void vr_tree_destroy(vr_tree* t) {
     cudaGetDevice(&prev);
     cudaSetDevice(t->device);
     cudaFree(t->nodes); cudaFree(t->extra);
-    cudaFree(t->wide); cudaFree(t->wslot); cudaFree(t->wrecs);
-    for (auto& kv : t->res) { cudaFree(kv.second.queues); cudaFree(kv.second.cam_ring); cudaFree(kv.second.opt_ring); }
+    cudaFree(t->wide); cudaFree(t->wslot); cudaFree(t->wrecs); cudaFree(t->sigma_grid); cudaFree(t->tab_org);
+    for (auto& kv : t->res) {
+        cudaFree(kv.second.queues); cudaFree(kv.second.cam_ring); cudaFree(kv.second.opt_ring); cudaFree(kv.second.tile_mask);
+    }
     for (int i = 0; i < vr_tree::HostPath::kRing; ++i) {
         cudaFree(t->host.buf[i]);
         if (t->host.rendered[i]) cudaEventDestroy(t->host.rendered[i]);
@@ -451,13 +453,23 @@ static int tree_create_impl(const vr_tree_desc* d, const vr_tree_quant_desc* q, 
     D.pos_scale = (float)(1u << (24 - wp));
     D.pos_hi = (1.f - 1e-6f) * D.pos_scale;   // exact: a power-of-two multiple of 0x3F7FFFEF
     D.icube_bias = 0x73000000u + ((uint32_t)wp << 23);
+    {
+        VR_CUDA(cudaMalloc(&t->tab_org, (size_t)n_tab * sizeof(uint4)));
+        VR_CUDA(cudaMalloc(&t->sigma_grid, (size_t)(kSigmaGridCells + 1) * 4));
+        const int n = build_sigma_grid(t, nullptr, true);
+        if (n < 0) return cuda_fail(cudaGetLastError(), "coarse sigma grid");
+        VR_CUDA(cudaDeviceSynchronize());
+        g_launches += n;
+        D.sigma_grid = t->sigma_grid;
+    }
     vr_tree_info& I = t->info;
     I.capacity = d->capacity; I.max_depth = D.max_depth; I.rec_bytes = rec_bytes;
     I.node_bytes = n_slots * 4; I.rec_total_bytes = n_slots * (long long)rec_bytes;
     I.top_bytes = 16 * 16 * 16 * 4;   // a dense 16^3 grid of node words
     I.kernel_basis = kbd; I.wide_parity = wp; I.n_tables = n_tab;
     I.wide_bytes = n_entries * 4; I.wrecs_bytes = n_entries * (long long)rec_bytes;
-    I.kernel_bytes = I.wide_bytes + I.wrecs_bytes;
+    I.grid_bytes = (long long)(kSigmaGridCells + 1) * 4 + (long long)n_tab * (long long)sizeof(uint4);
+    I.kernel_bytes = I.wide_bytes + I.wrecs_bytes + I.grid_bytes;
     I.device_bytes = I.kernel_bytes + (slot_map ? n_entries * 4 : 0);
     guard.ok = true;
     *out = t;
@@ -492,6 +504,11 @@ int vr_tree_update_data(vr_tree* t, const uint16_t* data_dev, void* stream) {
                                                                                             n_entries, rec_bytes, t->wide);
     VR_CUDA(cudaGetLastError());
     g_launches += 1;
+    {   // the coarse sigma grid from the new sigma bits, behind the table rewrite on the same stream
+        const int n = build_sigma_grid(t, (cudaStream_t)stream, false);
+        if (n < 0) return cuda_fail(cudaGetLastError(), "coarse sigma grid");
+        g_launches += n;
+    }
     {
         std::lock_guard<std::mutex> lk(t->res_mu);
         ++t->data_gen;

@@ -1,5 +1,6 @@
 // vr_tree.h -- the device tree behind the C-ABI's vr_tree handle and the CUDA error channel, shared by the tree's
-// construction (vr_tree.cu) and the launch entry points (vr_api.cu).  No other file includes it.
+// construction (vr_tree.cu), its coarse sigma grid and the tile-coverage pass (vr_cull.cu) and the launch entry points
+// (vr_api.cu).  No other file includes it.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -13,7 +14,9 @@
 
 namespace vrb {
 
-// Kernel launches so far (vr_launch_count): every entry point adds the launches it makes.
+// Kernel launches so far (vr_launch_count): every entry point adds the launches it makes, except that a batch
+// render's tile-coverage pass is counted with the march it prepares -- one count per march launch, as callers that
+// budget launches per batch (one march per chunk) have always seen it.
 extern std::atomic<unsigned long long> g_launches;
 
 // The device check of every entry point.  With a tree, the current device must be the tree's (cudaGetDevice only, so
@@ -35,6 +38,16 @@ inline int cuda_fail(cudaError_t e, const char* what, const char* where = "") {
     return fail(e == cudaErrorMemoryAllocation ? VR_ENOMEM : VR_ECUDA, "%s: %s%s", what, cudaGetErrorString(e), where);
 }
 
+// The coarse sigma grid of a tree from its tables (vr_cull.cu), ordered on `stream`.  with_org: first the origin of
+// every table into t->tab_org (tree creation); without, the origins of the creation are reused (vr_tree_update_data,
+// which changes sigma only).  Returns the number of kernels launched, or a negative value on a CUDA error.
+int build_sigma_grid(vr_tree* t, cudaStream_t stream, bool with_org);
+
+// The tile-coverage pass of a batch launch (vr_cull.cu): writes the tile mask of P's n_views views into the stream's
+// mask buffer and sets P.tile_mask / P.mask_words.  P holds the tree, the staged cameras and options and the work
+// decomposition's tiles_x / tiles_y.
+int launch_tile_mask(vr_tree* t, LaunchDev& P, cudaStream_t stream);
+
 }  // namespace vrb
 
 #define VR_STR_(x) #x
@@ -53,6 +66,8 @@ struct StreamRes {
     vrb::CamDev* cam_ring = nullptr; // kCamRing entries; batches take consecutive slots
     vrb::OptDev* opt_ring = nullptr; // kCamRing entries beside cam_ring (same slots), allocated by the first
                                      // batch with options per view
+    uint32_t* tile_mask = nullptr;   // tile coverage of the batch march launches on this stream (vr_cull.cu)
+    size_t mask_cap = 0;             // its size in words
     unsigned int next_queue = 0, cam_pos = 0;
     unsigned long long data_gen = 0; // the tree's data_gen at this stream's last march launch
 };
@@ -69,6 +84,8 @@ struct vr_tree {
     uint32_t* nodes = nullptr;
     uint32_t* wslot = nullptr;
     long long n_tables = 0;
+    uint32_t* sigma_grid = nullptr;   // coarse sigma grid (TreeDev::sigma_grid)
+    uint4* tab_org = nullptr;         // origin and level of every table (vr_cull.cu), kept for grid rebuilds
     std::mutex res_mu;
     std::unordered_map<cudaStream_t, StreamRes> res;
     // bumped (under res_mu) by every vr_tree_update_data: a stream's first march launch after an update is made

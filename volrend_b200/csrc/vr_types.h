@@ -44,7 +44,24 @@ struct TreeDev {
     float pos_scale;        // 2^(24 - wide_p)
     float pos_hi;           // (1 - 1e-6f) * pos_scale: upper clamp of a position (n3tree_query.hpp:17-19)
     uint32_t icube_bias;    // 0x73000000 + (wide_p << 23): 1/2^depth = bits(icube_bias - (w & 0x7f800000))
+    // coarse sigma grid (vr_cull.cu, built at tree creation): kSigmaGridN^3 cells over the unit cube, x slowest, each the largest fp16 sigma of
+    // the reachable leaves that overlap it as a sigma_key; then the key of the smallest sigma of every leaf.  Read only
+    // by the tile-coverage pass of batch launches (vr_cull.cu).
+    const uint32_t* sigma_grid;
 };
+
+// Level of the coarse sigma grid: 2^5 = 32 cells per axis (DESIGN.md 3).
+constexpr int kSigmaGridLevel = 5, kSigmaGridN = 1 << kSigmaGridLevel;
+constexpr int kSigmaGridCells = kSigmaGridN * kSigmaGridN * kSigmaGridN;
+
+// Order-preserving map of a non-NaN float to u32 (-0 below +0): unsigned max / min of keys is float max / min, and
+// key 0 is below every float, so a zeroed grid is "no leaf yet".
+__host__ __device__ inline uint32_t sigma_key(uint32_t fbits) {
+    return (fbits & 0x80000000u) ? ~fbits : (fbits | 0x80000000u);
+}
+__host__ __device__ inline uint32_t sigma_key_bits(uint32_t key) {
+    return (key & 0x80000000u) ? (key & 0x7fffffffu) : ~key;
+}
 
 struct CamDev {
     int32_t width, height;
@@ -123,6 +140,11 @@ struct LaunchDev {
     // error and the caller's per-slot sums.  Last, as above.
     const float* err;
     float* score;
+    // tile coverage of batch launches (vr_cull.cu): bit ty * tiles_x + tx of view v's mask_words words is clear when no
+    // ray of that tile can shade a sample; nullptr = every tile is marched.  Read only by the uninstrumented product
+    // instantiations (kOutLinear, kOutSurface, kOutViewOpts).  Last, as above.
+    const uint32_t* tile_mask;
+    int32_t mask_words;
 };
 
 }  // namespace vrb
