@@ -34,7 +34,7 @@ $(OBJ)/vr_kernels_%.o: volrend_b200/csrc/vr_kernels_inst.cu volrend_b200/csrc/vr
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -DVR_KBD=$* -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_$*.log || (cat $(OBJ)/ptxas_$*.log; false)
 
-$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_tree.h volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h volrend_b200/csrc/vr_query.h volrend_b200/csrc/vr_tv.h include/volrend_b200.h
+$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_tree.h volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h volrend_b200/csrc/vr_query.h volrend_b200/csrc/vr_tv.h volrend_b200/csrc/vr_build.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -62,6 +62,10 @@ $(OBJ)/vr_normals.o: volrend_b200/csrc/vr_normals.cu volrend_b200/csrc/vr_normal
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_normals.log || (cat $(OBJ)/ptxas_normals.log; false)
 
+$(OBJ)/vr_build.o: volrend_b200/csrc/vr_build.cu volrend_b200/csrc/vr_build.h
+	@mkdir -p $(OBJ)
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_build.log || (cat $(OBJ)/ptxas_build.log; false)
+
 $(OBJ)/vr_quant.o: volrend_b200/csrc/vr_quant.cu volrend_b200/csrc/vr_quant.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_quant.log || (cat $(OBJ)/ptxas_quant.log; false)
@@ -82,7 +86,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp volrend_b200/csrc/vr_frames.h incl
 	@mkdir -p $(OBJ)
 	$(CXX) -O3 -std=c++17 -fPIC -Iinclude -c $< -o $@
 
-$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_cull.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_tv.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
+$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_cull.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_tv.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_build.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
 oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/liberror_oracle.so oracle/libsurface_harness.so

@@ -461,6 +461,26 @@ int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim
                      int32_t bits, uint16_t* quant_colors_dev, uint16_t* quant_map_dev, uint16_t* sigma_dev,
                      uint16_t* data_retained_dev, int64_t* n_kept_out, void* stream);
 
+/* ---- tree construction (volrend_b200/csrc/vr_build.cu) ----------------------------------------------------
+ * The canonical N3Tree of a set of voxel cells; DESIGN.md section 21 states it bit for bit.  cells_dev: int32 [n][4],
+ * (level, i, j, k), the cube [i, i+1) x [j, j+1) x [k, k+1) * 2^-level of the tree's unit cube with 1 <= level <= 23
+ * and 0 <= i, j, k < 2^level (i along x, the first axis of child[node, x, y, z]); rows_dev: fp16 [n][data_dim], laid
+ * out as a row of N3Tree::data_.  The tree holds the root and one node per cell of level >= 1 that strictly contains a
+ * listed cell; listed slots hold their rows bit for bit, every other slot +0.  Nodes are numbered breadth first, the
+ * nodes of a level in Morton order (x the most significant bit), links are positive offsets: the output depends only
+ * on the set of cells.  With VR_BUILD_MERGE, bottom-up, a node whose 8 slots are leaves with bitwise-equal rows (an
+ * unlisted slot reads +0) becomes a leaf of its parent with that row; the root stays.
+ * child_dev and data_dev both NULL: only *n_nodes_out is written.  Otherwise child_dev int32 [max_nodes*8] and data_dev
+ * fp16 [max_nodes*8*data_dim] (caller-owned) receive the tree's first n_nodes nodes.  The node count synchronises
+ * `stream` once; the rest is stream-ordered, with scratch from the device's default stream-ordered pool.  VR_EINVAL,
+ * with nothing written, for: a level outside [1, 23], a coordinate outside [0, 2^level), a duplicate or overlapping
+ * cell, n outside [0, INT32_MAX], data_dim < 1, NULL cells_dev / rows_dev with n > 0, NULL n_nodes_out, only one of
+ * child_dev / data_dev NULL, a buffer that is not device memory of the current device, more than 0xffffffff / 8 nodes
+ * (the int32 links and the u32 slot map) and more nodes than max_nodes. */
+#define VR_BUILD_MERGE 1u
+int vr_tree_build(const int32_t* cells_dev, const uint16_t* rows_dev, int64_t n, int32_t data_dim, uint32_t flags,
+                  int32_t* child_dev, uint16_t* data_dev, int64_t max_nodes, int64_t* n_nodes_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

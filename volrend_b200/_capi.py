@@ -16,6 +16,7 @@ VR_BASIS_MAX = 25
 VR_OK, VR_EINVAL, VR_ENODEVICE, VR_ECUDA, VR_ENOMEM, VR_EUNSUPPORTED = 0, -1, -2, -3, -4, -5
 VR_FMT_RGBA, VR_FMT_SH, VR_FMT_SG, VR_FMT_ASG = 0, 1, 2, 3
 VR_TREE_SLOT_MAP = 1
+VR_BUILD_MERGE = 1
 
 
 class vr_tree_desc(C.Structure):
@@ -148,6 +149,8 @@ SYMBOLS = {
     "vr_mesh_estimate_normals": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "vr_tree_compress": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "vr_tree_build": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
 }
 
 _lib = None

@@ -15,6 +15,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "vr_build.h"
 #include "vr_frames.h"
 #include "vr_kernels.h"
 #include "vr_normals.h"
@@ -1024,6 +1025,52 @@ int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim
     if (reject == kQuantTooManyPoints)
         return fail(VR_EINVAL, "%lld kept voxels x %d quantised basis functions exceed %d points", kept, n_quant, INT32_MAX);
     *n_kept_out = kept;
+    return VR_OK;
+}
+
+// Canonical tree of a set of voxel cells (kernels: vr_build.cu).
+int vr_tree_build(const int32_t* cells_dev, const uint16_t* rows_dev, int64_t n, int32_t data_dim, uint32_t flags,
+                  int32_t* child_dev, uint16_t* data_dev, int64_t max_nodes, int64_t* n_nodes_out, void* stream) {
+    if (!n_nodes_out) return fail(VR_EINVAL, "null n_nodes_out");
+    if (n < 0 || n > INT32_MAX) return fail(VR_EINVAL, "n %lld outside [0, %d]", (long long)n, INT32_MAX);
+    if (data_dim < 1) return fail(VR_EINVAL, "data_dim %d < 1", data_dim);
+    if (flags & ~VR_BUILD_MERGE) return fail(VR_EINVAL, "unknown flags 0x%x", flags);
+    if (n > 0 && (!cells_dev || !rows_dev)) return fail(VR_EINVAL, "null cells_dev or rows_dev with n = %lld", (long long)n);
+    if ((child_dev == nullptr) != (data_dev == nullptr))
+        return fail(VR_EINVAL, "child_dev and data_dev must both be NULL (count only) or both be given");
+    if (int rc = need_device(nullptr)) return rc;
+    int dev = 0;
+    VR_CUDA(cudaGetDevice(&dev));
+    const struct { const void* p; const char* name; } bufs[] = {
+        {cells_dev, "cells_dev"}, {rows_dev, "rows_dev"}, {child_dev, "child_dev"}, {data_dev, "data_dev"}};
+    for (const auto& b : bufs) {
+        if (!b.p) continue;
+        cudaPointerAttributes pa{};
+        if (cudaPointerGetAttributes(&pa, b.p) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(VR_EINVAL, "%s is not a CUDA allocation", b.name);
+        }
+        if ((pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged) || pa.device != dev)
+            return fail(VR_EINVAL, "%s is not device memory of the current device %d", b.name, dev);
+    }
+    BuildArgs a{};
+    a.cells = cells_dev; a.rows = rows_dev; a.n = n; a.data_dim = data_dim; a.merge = (flags & VR_BUILD_MERGE) != 0;
+    a.child = child_dev; a.data = data_dev; a.max_nodes = max_nodes; a.node_limit = 0xffffffffll / 8;
+    long long nodes = 0;
+    int reject = kBuildOk, launches = 0;
+    const cudaError_t e = tree_build(a, (cudaStream_t)stream, &nodes, &reject, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) return cuda_fail(e, "tree build");
+    switch (reject) {
+        case kBuildBadCell: return fail(VR_EINVAL, "a cell has a level outside [1, 23] or a coordinate outside [0, 2^level)");
+        case kBuildOverlap: return fail(VR_EINVAL, "two cells are equal or one contains the other");
+        case kBuildTooLarge:
+            return fail(VR_EINVAL, "the tree has %lld nodes: more than the %lld the int32 links and the u32 slot map address",
+                        nodes, a.node_limit);
+        case kBuildCapacity: return fail(VR_EINVAL, "the tree has %lld nodes, the outputs room for %lld", nodes, (long long)max_nodes);
+        default: break;
+    }
+    *n_nodes_out = nodes;
     return VR_OK;
 }
 
