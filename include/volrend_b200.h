@@ -481,6 +481,20 @@ int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim
 int vr_tree_build(const int32_t* cells_dev, const uint16_t* rows_dev, int64_t n, int32_t data_dim, uint32_t flags,
                   int32_t* child_dev, uint16_t* data_dev, int64_t max_nodes, int64_t* n_nodes_out, void* stream);
 
+/* ---- image quality (volrend_b200/csrc/vr_ssim.cu) ------------------------------------------------------
+ * Per-view SSIM of x against y, JaxNeRF's compute_ssim (DESIGN.md section 22): an 11-tap Gaussian (sigma 1.5,
+ * normalised) applied separably with valid filtering to x, y, x^2, y^2 and xy of each of channels 0..2, clipped
+ * variances and covariance, C1 = 0.01^2, C2 = 0.03^2, max_val 1, no clamping; ssim_dev[v] (double) is the mean over the
+ * 3 channels and the (height-10) x (width-10) valid pixels of view v, overwritten.  x_dev: float32
+ * [n_views][height][width][x_channels], y_dev the same with y_channels; channels 3 or 4 (only 0..2 are read).  dx_dev
+ * NULL: forward only; otherwise x's layout, and dx += dx_scale * d ssim_v / dx on channels 0..2 of every view (other
+ * elements untouched).  Bit-reproducible from run to run (no atomics).  Asynchronous on stream, with scratch from the
+ * device's default stream-ordered pool.  n_views = 0 launches nothing.  VR_EINVAL for n_views < 0, height or width
+ * below 11, channels other than 3 or 4, a non-finite dx_scale, NULL x_dev, y_dev or ssim_dev, and buffers that are not
+ * device memory of the current device. */
+int vr_image_ssim(const float* x_dev, int x_channels, const float* y_dev, int y_channels, int n_views, int height,
+                  int width, double* ssim_dev, float* dx_dev, float dx_scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,8 +9,9 @@ For the default flags (--bits 16 --sigma_thresh 2.0 --retain 1) and for --retain
   * host time to assemble the dict, deflate and write it (np.savez_compressed), median of --host-reps runs;
   * input file size (np.savez, as training writes it) and compressed size.
 Also: the numpy restatement of the contract (oracle/quant_oracle.py, not svox) timed on one point set of the same
-tree and checked equal to the device output for that set, and the PSNR of --views views rendered at 800x800 from the
-compressed tree against the original (the stand-in's colours are random, so this says little about real scenes).
+tree and checked equal to the device output for that set, and the PSNR and SSIM (volrend_b200.evaluate) of --views
+views rendered at 800x800 from the compressed tree against the original (the stand-in's colours are random, so this
+says little about real scenes).
 
 Prints the card name and power limit, then one JSON line.  Writes only to a temporary directory."""
 import argparse
@@ -90,11 +91,6 @@ def stage_kernel_ms(flat, dd, retain, bits, thresh, tmp):
     return {k: round(v, 3) for k, v in out.items()}
 
 
-def psnr(a, b):
-    mse = float(np.mean((np.clip(a, 0, 1).astype(np.float64) - np.clip(b, 0, 1)) ** 2))
-    return float("inf") if mse == 0 else float(-10.0 * np.log10(mse))
-
-
 def render_views(tree, views):
     import torch
     from volrend_b200 import Camera, RenderOptions, launch_renderer, synth
@@ -122,8 +118,10 @@ def main():
     import torch
     import compress_cases as cc
     from oracle import quant_oracle as qo
-    from volrend_b200 import N3Tree, compress_npz, synth
+    from volrend_b200 import N3Tree, RenderOptions, compress_npz, evaluate, synth
     from volrend_b200.compress import _write_npz
+    from volrend_b200.evaluate import psnr
+    from volrend_b200.views import cameras
     c = card()
     print("card:", c, flush=True)
     torch.cuda.init()
@@ -173,10 +171,14 @@ def main():
             ref = render_views(orig, args.views)
             orig.free_cuda()
             comp = N3Tree(out)
-            got = render_views(comp, args.views)
+            poses = synth.nerf_synthetic_test_poses(200)
+            cams = cameras([poses[i] for i in args.views], 800, 800, synth.focal_for(800), synth.focal_for(800))
+            mse, ssim = evaluate(comp, cams, ref, RenderOptions())
             comp.free_cuda()
-            row["psnr_db"] = [round(psnr(a, b), 2) for a, b in zip(got, ref)]
-            print(f"retain {retain} PSNR vs original (views {args.views}): {row['psnr_db']}", flush=True)
+            row["psnr_db"] = [round(float(p), 2) for p in psnr(mse)]
+            row["ssim"] = [round(float(v), 4) for v in ssim]
+            print(f"retain {retain} PSNR / SSIM vs original (views {args.views}): {row['psnr_db']} / {row['ssim']}",
+                  flush=True)
             torch.cuda.empty_cache()
     print(json.dumps(res), flush=True)
 

@@ -6,8 +6,8 @@ collapse:
   * leaves and nodes before and after, device_bytes of the loaded tree;
   * config-2 Mrays/s of the pruned tree against the original (vr_render_batch of the 200 views, CUDA events, median
     of --reps after --warmup, trees alternated);
-  * PSNR of the pruned tree's renders against the original's on --psnr-views poses NOT used for the weights (the
-    orbit shifted by half a step);
+  * PSNR and SSIM (volrend_b200.evaluate) of the pruned tree's renders against the original's on --psnr-views poses
+    NOT used for the weights (the orbit shifted by half a step);
   * compressed file size (compress_npz defaults + deflate) with and without pruning.
 Also the weights pass itself: ms per view next to the render ms per view of the same batch, alternated.
 
@@ -21,8 +21,6 @@ import subprocess
 import sys
 import tempfile
 import time
-
-import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -53,11 +51,6 @@ def events_ms(fn, warmup, reps):
     return statistics.median(out)
 
 
-def psnr(a, b):
-    mse = float(np.mean((np.clip(a, 0, 1).astype(np.float64) - np.clip(b, 0, 1)) ** 2))
-    return float("inf") if mse == 0 else float(-10.0 * np.log10(mse))
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--depth", type=int, default=10)
@@ -68,8 +61,9 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     import torch
-    from volrend_b200 import N3Tree, RenderOptions, compress_npz, leaf_weights, prune_npz, render_batch, synth
+    from volrend_b200 import N3Tree, RenderOptions, compress_npz, evaluate, leaf_weights, prune_npz, render_batch, synth
     from volrend_b200.compress import _write_npz
+    from volrend_b200.evaluate import psnr
     from volrend_b200.views import cameras
     c = card()
     print("card:", c, flush=True)
@@ -154,14 +148,15 @@ def main():
                 for _ in range(2):          # alternated
                     ms_o.append(render_ms(base))
                     ms_p.append(render_ms(pt))
-                frames = held_frames(pt)
+                mse, ssim = evaluate(pt, held, ref_frames, opt)
                 row = dict(thresh=thresh, collapse=collapse, prune_host_s=round(prune_s, 2),
                            leaves_kept=int((leaf & (weights >= thresh)).sum()),
                            leaves_after=int((pz["child"].reshape(-1) == 0).sum()), nodes_after=int(pz["child"].shape[0]),
                            device_bytes=pt.info()["device_bytes"],
                            mrays_original=[round(W * H * 200 / m / 1e3, 1) for m in ms_o],
                            mrays_pruned=[round(W * H * 200 / m / 1e3, 1) for m in ms_p],
-                           psnr_db_held_out=[round(psnr(a, b), 2) for a, b in zip(frames, ref_frames)])
+                           psnr_db_held_out=[round(float(p), 2) for p in psnr(mse)],
+                           ssim_held_out=[round(float(v), 4) for v in ssim])
                 pt.free_cuda()
                 if not args.no_sizes:
                     p = os.path.join(tmp, "pruned.npz")

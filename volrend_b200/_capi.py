@@ -151,6 +151,8 @@ SYMBOLS = {
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "vr_tree_build": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p,
                                 C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
+    "vr_image_ssim": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                C.c_void_p, C.c_float, C.c_void_p]),
 }
 
 _lib = None

@@ -23,6 +23,7 @@
 #include "vr_quant.h"
 #include "vr_query.h"
 #include "vr_raster.h"
+#include "vr_ssim.h"
 #include "vr_tree.h"
 #include "vr_tv.h"
 #include "vr_wire.h"
@@ -901,6 +902,26 @@ int ensure_wire_levels(const vr_tree* t, const WireTree& w, cudaStream_t stream)
     }
     return VR_OK;
 }
+// VR_EINVAL unless every non-null buffer is device (or managed) memory of the current device.
+struct NamedBuffer {
+    const void* p;
+    const char* name;
+};
+int current_device_buffers(std::initializer_list<NamedBuffer> bufs) {
+    int dev = 0;
+    VR_CUDA(cudaGetDevice(&dev));
+    for (const auto& b : bufs) {
+        if (!b.p) continue;
+        cudaPointerAttributes pa{};
+        if (cudaPointerGetAttributes(&pa, b.p) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(VR_EINVAL, "%s is not a CUDA allocation", b.name);
+        }
+        if ((pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged) || pa.device != dev)
+            return fail(VR_EINVAL, "%s is not device memory of the current device %d", b.name, dev);
+    }
+    return VR_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1039,20 +1060,9 @@ int vr_tree_build(const int32_t* cells_dev, const uint16_t* rows_dev, int64_t n,
     if ((child_dev == nullptr) != (data_dev == nullptr))
         return fail(VR_EINVAL, "child_dev and data_dev must both be NULL (count only) or both be given");
     if (int rc = need_device(nullptr)) return rc;
-    int dev = 0;
-    VR_CUDA(cudaGetDevice(&dev));
-    const struct { const void* p; const char* name; } bufs[] = {
-        {cells_dev, "cells_dev"}, {rows_dev, "rows_dev"}, {child_dev, "child_dev"}, {data_dev, "data_dev"}};
-    for (const auto& b : bufs) {
-        if (!b.p) continue;
-        cudaPointerAttributes pa{};
-        if (cudaPointerGetAttributes(&pa, b.p) != cudaSuccess) {
-            cudaGetLastError();
-            return fail(VR_EINVAL, "%s is not a CUDA allocation", b.name);
-        }
-        if ((pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged) || pa.device != dev)
-            return fail(VR_EINVAL, "%s is not device memory of the current device %d", b.name, dev);
-    }
+    if (int rc = current_device_buffers({{cells_dev, "cells_dev"}, {rows_dev, "rows_dev"}, {child_dev, "child_dev"},
+                                         {data_dev, "data_dev"}}))
+        return rc;
     BuildArgs a{};
     a.cells = cells_dev; a.rows = rows_dev; a.n = n; a.data_dim = data_dim; a.merge = (flags & VR_BUILD_MERGE) != 0;
     a.child = child_dev; a.data = data_dev; a.max_nodes = max_nodes; a.node_limit = 0xffffffffll / 8;
@@ -1071,6 +1081,26 @@ int vr_tree_build(const int32_t* cells_dev, const uint16_t* rows_dev, int64_t n,
         default: break;
     }
     *n_nodes_out = nodes;
+    return VR_OK;
+}
+
+// Per-view SSIM and its gradient (kernels: vr_ssim.cu).
+int vr_image_ssim(const float* x_dev, int x_channels, const float* y_dev, int y_channels, int n_views, int height,
+                  int width, double* ssim_dev, float* dx_dev, float dx_scale, void* stream) {
+    if (n_views < 0) return fail(VR_EINVAL, "n_views %d < 0", n_views);
+    if (height < 11 || width < 11) return fail(VR_EINVAL, "images are %dx%d: SSIM needs at least 11x11", width, height);
+    if ((x_channels != 3 && x_channels != 4) || (y_channels != 3 && y_channels != 4))
+        return fail(VR_EINVAL, "channels %d and %d: each must be 3 or 4", x_channels, y_channels);
+    if (!std::isfinite(dx_scale)) return fail(VR_EINVAL, "dx_scale %g is not finite", dx_scale);
+    if (!x_dev || !y_dev || !ssim_dev) return fail(VR_EINVAL, "null x_dev, y_dev or ssim_dev");
+    if (int rc = need_device(nullptr)) return rc;
+    if (int rc = current_device_buffers({{x_dev, "x_dev"}, {y_dev, "y_dev"}, {ssim_dev, "ssim_dev"}, {dx_dev, "dx_dev"}}))
+        return rc;
+    int launches = 0;
+    const cudaError_t e = ssim_pass(x_dev, x_channels, y_dev, y_channels, n_views, height, width, ssim_dev, dx_dev,
+                                    dx_scale, (cudaStream_t)stream, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) return cuda_fail(e, "image SSIM");
     return VR_OK;
 }
 

@@ -5,7 +5,7 @@
                                     [--step_size S] [--sigma_thresh S] [--stop_thresh S] [--background B]
                                     [--steps 100] [--lr 1e-2] [--batch 4] [--seed 0] [--holdout K]
                                     [--refine-every K] [--refine-fraction 0.1] [--max-depth 23]
-                                    [--tv-sigma 0] [--tv-color 0]
+                                    [--tv-sigma 0] [--tv-color 0] [--dssim-weight 0]
 
 The fit uses the march's own samples: the renders are ``render_batch``'s float output and the gradients come from the
 same samples on the GPU (``vr_tree_leaf_grads``, see :func:`volrend_b200.leaf_grads`; formulas in DESIGN.md section
@@ -15,7 +15,8 @@ step on the master and writes it, rounded to fp16, into the device tree (``N3Tre
 changes only with ``--refine-every K``: every K steps the leaves that carry the most residual error are split
 (coarse-to-fine, :mod:`volrend_b200.refine`, DESIGN.md section 19).  ``--tv-sigma`` / ``--tv-color`` add a
 total-variation prior between neighbouring leaves to the gradient (:func:`volrend_b200.leaf_tv`, DESIGN.md section 20),
-which keeps the many small leaves of a refined tree from fitting each training ray on its own.  Columns the device does not keep (coefficients of a basis size without its own kernel beyond the first, and
+which keeps the many small leaves of a refined tree from fitting each training ray on its own.  ``--dssim-weight``
+adds a structural term, lambda * (1 - SSIM), to the step loss (:func:`volrend_b200.image_ssim`, DESIGN.md section 22).  Columns the device does not keep (coefficients of a basis size without its own kernel beyond the first, and
 SG / ASG lobes) get no gradient and keep their values.
 
 Targets are one PNG per pose or one ``.npy`` of shape [V, H, W, 3 | 4], uint8 or float in [0, 1].  RGBA targets are
@@ -33,6 +34,7 @@ import sys
 import numpy as np
 
 from .compress import _write_npz, carried_keys, check_uncompressed
+from .evaluate import evaluate
 from .views import add_view_arguments, open_inputs, target_batch
 
 _ADVICE = "fine-tune the uncompressed tree first, then prune and compress"
@@ -40,7 +42,7 @@ _ADVICE = "fine-tune the uncompressed tree first, then prune and compress"
 
 def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int, seed: int, on_step=None,
              refine_every: int = 0, refine_fraction: float = 0.1, max_depth: int = 23, on_refine=None,
-             tv_sigma: float = 0.0, tv_color: float = 0.0):
+             tv_sigma: float = 0.0, tv_color: float = 0.0, dssim_weight: float = 0.0):
     """Fits the leaf data of ``tree`` (an ``N3Tree`` loaded with ``load_cuda(slot_map=True)`` that still holds its host
     data) to ``targets``: a sequence of one image per camera in ``cams`` ([H, W, 3 | 4], uint8 or float, indexed
     lazily, so it may read files on demand).  Each of ``steps`` steps takes the next ``batch`` views of a shuffle seeded
@@ -59,15 +61,19 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
     Total variation: with ``tv_sigma`` or ``tv_color`` > 0, every step adds the gradient of the TV prior of the master
     (:func:`volrend_b200.leaf_tv`, weights ``tv_sigma`` for sigma and ``tv_color`` for the colour coefficients) to the
     image gradient before the Adam step.  The neighbour table (:func:`volrend_b200.leaf_neighbors`) is built before
-    the first step and again after every refinement that splits leaves.  ``losses`` and ``on_step`` stay the MSE."""
+    the first step and again after every refinement that splits leaves.  ``losses`` and ``on_step`` stay the MSE.
+
+    D-SSIM: with ``dssim_weight`` = lambda > 0 the step loss is ``MSE + lambda * (1 - mean over the batch of ssim_v)``
+    (:func:`volrend_b200.image_ssim`); its gradient is added to the per-pixel gradient before the leaf pass.
+    ``losses`` and ``on_step`` stay the MSE."""
     import torch
-    from .host import leaf_grads, leaf_neighbors, leaf_tv, render_batch
+    from .host import image_ssim, leaf_grads, leaf_neighbors, leaf_tv, render_batch
     from .refine import leaf_scores, refine_plan
     if steps < 0 or batch < 1:
         raise ValueError(f"steps {steps} must be >= 0 and batch {batch} >= 1")
     if refine_every < 0:
         raise ValueError(f"refine_every {refine_every} must be >= 0")
-    for name, w in (("tv_sigma", tv_sigma), ("tv_color", tv_color)):
+    for name, w in (("tv_sigma", tv_sigma), ("tv_color", tv_color), ("dssim_weight", dssim_weight)):
         if not (float(w) >= 0.0) or math.isinf(float(w)):
             raise ValueError(f"{name} {w} must be finite and >= 0")
     tv = tv_sigma > 0 or tv_color > 0
@@ -77,8 +83,10 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
         raise ValueError("no views to fit")
     if tree.data_ is None:
         raise ValueError("the tree holds no host data to start from")
-    dev = torch.device("cuda", tree._device)
     H, W = cams[0].height, cams[0].width
+    if dssim_weight > 0 and min(H, W) < 11:
+        raise ValueError(f"dssim_weight {dssim_weight} needs images of at least 11x11 (the SSIM window), not {W}x{H}")
+    dev = torch.device("cuda", tree._device)
     master = torch.tensor(np.asarray(tree.data_, np.float32), device=dev).requires_grad_(True)
     opt = torch.optim.Adam([master], lr=lr)
     gen = np.random.default_rng(seed)
@@ -117,6 +125,8 @@ def finetune(tree, cams, targets, options, *, steps: int, lr: float, batch: int,
         diff = fo[..., :3] - tgt
         loss = diff.square().mean()
         dpix[..., :3] = diff * (2.0 / diff.numel())
+        if dssim_weight > 0:
+            image_ssim(fo, tgt, dx=dpix, dx_scale=-dssim_weight / nb)
         grad.zero_()
         leaf_grads(tree, vc, options, dpix, out=grad)
         if tv:
@@ -187,22 +197,16 @@ def _parser() -> argparse.ArgumentParser:
                     help="weight of the total-variation prior on sigma between neighbouring leaves (0: none)")
     ap.add_argument("--tv-color", type=float, default=0.0,
                     help="weight of the total-variation prior on the colour coefficients (0: none)")
+    ap.add_argument("--dssim-weight", type=float, default=0.0,
+                    help="weight lambda of the structural loss term lambda * (1 - SSIM) (0: MSE only)")
     return ap
 
 
 def _psnr(tree, cams, targets, idx, options) -> float:
-    import torch
-    from .host import render_batch
-    dev = torch.device("cuda", tree._device)
-    se, n = 0.0, 0
-    for v in idx:
-        H, W = cams[v].height, cams[v].width
-        fo = torch.empty((1, H, W, 4), dtype=torch.float32, device=dev)
-        render_batch(tree, [cams[v]], options, None, float_out=fo)
-        d = fo[..., :3] - target_batch(targets, [v], options.background_brightness, dev, H, W)
-        se += float(d.square().sum())
-        n += d.numel()
-    return -10.0 * math.log10(max(se / n, 1e-30))
+    """The PSNR of the pooled squared error over the views ``idx``: they share one size, so the pooled MSE is the
+    mean of the per-view MSE."""
+    mse, _ = evaluate(tree, [cams[v] for v in idx], [targets[v] for v in idx], options, ssim=False)
+    return -10.0 * math.log10(max(float(mse.mean()), 1e-30))
 
 
 def main(argv=None) -> int:
@@ -220,9 +224,11 @@ def main(argv=None) -> int:
         ap.error(f"--refine-fraction {args.refine_fraction} must be in [0, 1]")
     if args.max_depth < 1:
         ap.error(f"--max-depth {args.max_depth} < 1")
-    for flag, w in (("--tv-sigma", args.tv_sigma), ("--tv-color", args.tv_color)):
+    for flag, w in (("--tv-sigma", args.tv_sigma), ("--tv-color", args.tv_color), ("--dssim-weight", args.dssim_weight)):
         if not (w >= 0.0) or math.isinf(w):
             ap.error(f"{flag} {w} must be a finite number >= 0")
+    if args.dssim_weight > 0 and min(args.width, args.height) < 11:
+        ap.error(f"--dssim-weight needs images of at least 11x11 (the SSIM window), not {args.width}x{args.height}")
     tree, cams, targets, d, opt = open_inputs(ap, args, _ADVICE, holdout=args.holdout)
     n_train = len(cams) - args.holdout
     held = list(range(n_train, len(cams)))
@@ -233,6 +239,7 @@ def main(argv=None) -> int:
                          on_step=lambda s, l: print(f"step {s}: loss {l:.6g}"),
                          refine_every=args.refine_every, refine_fraction=args.refine_fraction,
                          max_depth=args.max_depth, tv_sigma=args.tv_sigma, tv_color=args.tv_color,
+                         dssim_weight=args.dssim_weight,
                          on_refine=lambda s, n, a, b: print(f"refine before step {s}: split {n}, nodes {a} -> {b}"))
     if held:
         print(f"held-out PSNR after: {_psnr(tree, cams, targets, held, opt):.3f} dB")

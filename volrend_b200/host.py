@@ -802,6 +802,41 @@ def leaf_tv(tree: N3Tree, nbr, data, lambda_sigma: float, lambda_color: float, o
     return out, energy
 
 
+def image_ssim(x, y, out=None, dx=None, dx_scale: float = 1.0, stream=None):
+    """Per-view SSIM of the images ``x`` against ``y`` (vr_image_ssim, DESIGN.md section 22: JaxNeRF's
+    ``compute_ssim`` on channels 0..2, 11-tap Gaussian, valid filtering, max value 1): contiguous float32 CUDA tensors
+    ``[V, H, W, 3 | 4]`` on one device with the same V, H, W, e.g. ``render_batch``'s ``float_out`` and
+    :func:`volrend_b200.views.target_batch`; H and W at least 11.  Returns a float64 tensor [V] (``out``, V float64
+    elements on that device, is overwritten when given).  ``dx`` (x's shape): ``dx += dx_scale * dssim_v/dx`` on
+    channels 0..2 of every view, the gradient of each view's SSIM with respect to x; other elements keep their values.
+    Asynchronous on ``stream``; bit-reproducible from run to run."""
+    import torch
+    if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.shape[-1] not in (3, 4):
+        raise ValueError("x must be a [V, H, W, 3 | 4] tensor")
+    if not isinstance(y, torch.Tensor) or y.dim() != 4 or y.shape[-1] not in (3, 4) or y.shape[:3] != x.shape[:3]:
+        raise ValueError(f"y must be a [{', '.join(str(int(s)) for s in x.shape[:3])}, 3 | 4] tensor")
+    V, H, W, cx = (int(s) for s in x.shape)
+    if H < 11 or W < 11:
+        raise ValueError(f"images are {W}x{H}: SSIM needs at least 11x11")
+    if not math.isfinite(float(dx_scale)):
+        raise ValueError(f"dx_scale {dx_scale} must be finite")
+    dev = x.device
+    if dev.type != "cuda":
+        raise ValueError("x must be a CUDA tensor")
+    _check_tensor("x", x, torch.float32, x.numel(), dev)
+    _check_tensor("y", y, torch.float32, y.numel(), dev)
+    if out is None:
+        out = torch.empty(V, dtype=torch.float64, device=dev)
+    else:
+        _check_tensor("out", out, torch.float64, V, dev)
+    if dx is not None:
+        _check_tensor("dx", dx, torch.float32, x.numel(), dev)
+    with torch.cuda.device(dev):
+        check(lib().vr_image_ssim(x.data_ptr(), cx, y.data_ptr(), int(y.shape[-1]), V, H, W, out.data_ptr(),
+                                  dx.data_ptr() if dx is not None else None, float(dx_scale), _stream_ptr(stream)))
+    return out
+
+
 def _draw_probe_runs(tree: N3Tree, arr, options, oarr, tile, img, fo, s) -> None:
     """The probe discs of a batch rendered with options per view (``arr`` cameras, ``oarr`` their vr_options): one
     vr_draw_probe per run of consecutive views with the same probe settings."""
