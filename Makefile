@@ -34,7 +34,7 @@ $(OBJ)/vr_kernels_%.o: volrend_b200/csrc/vr_kernels_inst.cu volrend_b200/csrc/vr
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -DVR_KBD=$* -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_$*.log || (cat $(OBJ)/ptxas_$*.log; false)
 
-$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_tree.h volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h volrend_b200/csrc/vr_query.h volrend_b200/csrc/vr_tv.h volrend_b200/csrc/vr_build.h volrend_b200/csrc/vr_ssim.h include/volrend_b200.h
+$(OBJ)/vr_api.o: volrend_b200/csrc/vr_api.cu volrend_b200/csrc/vr_tree.h volrend_b200/csrc/vr_frames.h volrend_b200/csrc/vr_types.h volrend_b200/csrc/vr_kernels.h volrend_b200/csrc/vr_raster.h volrend_b200/csrc/vr_wire.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_normals.h volrend_b200/csrc/vr_quant.h volrend_b200/csrc/vr_query.h volrend_b200/csrc/vr_tv.h volrend_b200/csrc/vr_build.h volrend_b200/csrc/vr_ssim.h volrend_b200/csrc/vr_iso.h include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -82,6 +82,10 @@ $(OBJ)/vr_query.o: volrend_b200/csrc/vr_query.cu volrend_b200/csrc/vr_query.h vo
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_query.log || (cat $(OBJ)/ptxas_query.log; false)
 
+$(OBJ)/vr_iso.o: volrend_b200/csrc/vr_iso.cu volrend_b200/csrc/vr_iso.h volrend_b200/csrc/vr_iso_table.h volrend_b200/csrc/vr_probe.h volrend_b200/csrc/vr_lumisphere.cuh volrend_b200/csrc/vr_march.cuh volrend_b200/csrc/vr_types.h include/volrend_b200.h
+	@mkdir -p $(OBJ)
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(OBJ)/ptxas_iso.log || (cat $(OBJ)/ptxas_iso.log; false)
+
 $(OBJ)/vr_mg.o: volrend_b200/csrc/vr_mg.cu include/volrend_b200.h
 	@mkdir -p $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
@@ -90,7 +94,7 @@ $(OBJ)/vr_png.o: volrend_b200/csrc/vr_png.cpp volrend_b200/csrc/vr_frames.h incl
 	@mkdir -p $(OBJ)
 	$(CXX) -O3 -std=c++17 -fPIC -Iinclude -c $< -o $@
 
-$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_cull.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_tv.o $(OBJ)/vr_ssim.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_build.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
+$(LIB): $(OBJ)/vr_api.o $(OBJ)/vr_tree.o $(OBJ)/vr_cull.o $(OBJ)/vr_raster.o $(OBJ)/vr_wire.o $(OBJ)/vr_tv.o $(OBJ)/vr_ssim.o $(OBJ)/vr_normals.o $(OBJ)/vr_quant.o $(OBJ)/vr_build.o $(OBJ)/vr_probe.o $(OBJ)/vr_query.o $(OBJ)/vr_iso.o $(OBJ)/vr_mg.o $(OBJ)/vr_png.o $(KOBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -lz -lpthread
 
 oracle: oracle/liboracle.so oracle/libprobe_oracle.so oracle/libweights_oracle.so oracle/libgrads_oracle.so oracle/liberror_oracle.so oracle/libsurface_harness.so

@@ -481,6 +481,29 @@ int vr_tree_compress(const uint16_t* data_dev, int64_t n_child, int32_t data_dim
 int vr_tree_build(const int32_t* cells_dev, const uint16_t* rows_dev, int64_t n, int32_t data_dim, uint32_t flags,
                   int32_t* child_dev, uint16_t* data_dev, int64_t max_nodes, int64_t* n_nodes_out, void* stream);
 
+/* ---- surface extraction (volrend_b200/csrc/vr_iso.cu) -----------------------------------------------------
+ * Marching cubes over the tree's leaf sigma; DESIGN.md section 23 states it bit for bit.  The lattice has R = 2^depth
+ * points per axis at the unit coordinates (i + 0.5) / R, i along x, each the fp16 sigma of the leaf that holds it as a
+ * float (NaN 0, +-inf +-65504; leaves deeper than `depth` are point-sampled), padded with a layer of 0 on every side,
+ * so surfaces close at the tree's bounds.  A point is inside when its value is > level.  One vertex per lattice edge
+ * whose endpoints differ, numbered by owner point (the edge's lower endpoint) in C order of (i, j, k), then axis x, y,
+ * z; it lies where the linear interpolation crosses `level` (float32, round to nearest, no contraction), in world
+ * coordinates ((u - offset) / scale).  Faces are the triangles of the generated table (vr_iso_table.h), cube by cube
+ * in C order of the lower corner, uint32 index triples wound so that normals point outwards.  Vertices are 9-float
+ * Mesh rows: position, colour, normal (the normals of vr_mesh_estimate_normals).  With VR_ISO_COLOR each colour is
+ * vr_tree_eval's colour of the edge's inside endpoint along -normal, with opt's basis_minmax (opt may be NULL: the
+ * whole basis); otherwise (1, 1, 1).  vert_dev and faces_dev both NULL: only the counts are written.  Otherwise the call
+ * counts first, which synchronises `stream` once, and then fills vert_dev [max_verts][9] and faces_dev [max_faces][3]
+ * (caller-owned) stream-ordered, with scratch from the device's default stream-ordered pool.  Bit-reproducible.
+ * Nothing is written on a refusal; the counts are reported when they are known.  VR_EINVAL: depth outside [1, 11],
+ * a non-finite level or level <= 0, unknown flags, NULL count pointers, exactly one output NULL, outputs smaller than
+ * the counts, buffers that are not device memory of the tree's device.  VR_EUNSUPPORTED: NDC trees, VR_ISO_COLOR on
+ * the trees vr_tree_eval cannot colour, more than 2^31-1 vertices or face corners.  VR_ENODEVICE without a device. */
+#define VR_ISO_COLOR 1u
+int vr_tree_isosurface(const vr_tree* tree, int32_t depth, float level, const vr_options* opt, uint32_t flags,
+                       float* vert_dev, int64_t max_verts, uint32_t* faces_dev, int64_t max_faces,
+                       int64_t* n_verts_out, int64_t* n_faces_out, void* stream);
+
 /* ---- image quality (volrend_b200/csrc/vr_ssim.cu) ------------------------------------------------------
  * Per-view SSIM of x against y, JaxNeRF's compute_ssim (DESIGN.md section 22): an 11-tap Gaussian (sigma 1.5,
  * normalised) applied separably with valid filtering to x, y, x^2, y^2 and xy of each of channels 0..2, clipped

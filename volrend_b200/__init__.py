@@ -16,11 +16,12 @@ from .evaluate import evaluate
 from .refine import refine_npz, refine_plan
 from .build import build_arrays, build_npz, grid_cells, leaf_cells
 from .anim import AnimKF, animation_frames, render_animation
+from .isosurface import extract_mesh, isosurface_arrays, write_obj
 
 __all__ = ["N3Tree", "Camera", "RenderOptions", "VolumeRenderer", "DataFormat", "launch_renderer", "MultiGpuRenderer", "VR_MG_VIEWS", "VR_MG_TILES",
            "Mesh", "draw_meshes", "draw_meshes_batch", "estimate_normals", "compress_npz", "prune_arrays", "prune_npz", "leaf_weights",
            "leaf_grads", "leaf_neighbors", "leaf_tv", "image_ssim", "evaluate", "finetune", "finetune_npz", "leaf_error", "refine_plan", "refine_npz",
-           "build_arrays", "build_npz", "grid_cells", "leaf_cells",
+           "build_arrays", "build_npz", "grid_cells", "leaf_cells", "isosurface_arrays", "extract_mesh", "write_obj",
            "AnimKF", "animation_frames", "render_animation",
            "render_batch", "render_bands", "render_bands_batch", "render_frames_host", "render_frames_png", "write_png_file", "lib", "LIB_PATH", "VolrendError",
            "CAMERA_DEFAULT_FOCAL_LENGTH", "VOLREND_GLOBAL_BASIS_MAX"]

@@ -17,6 +17,7 @@ VR_OK, VR_EINVAL, VR_ENODEVICE, VR_ECUDA, VR_ENOMEM, VR_EUNSUPPORTED = 0, -1, -2
 VR_FMT_RGBA, VR_FMT_SH, VR_FMT_SG, VR_FMT_ASG = 0, 1, 2, 3
 VR_TREE_SLOT_MAP = 1
 VR_BUILD_MERGE = 1
+VR_ISO_COLOR = 1
 
 
 class vr_tree_desc(C.Structure):
@@ -151,6 +152,9 @@ SYMBOLS = {
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "vr_tree_build": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p,
                                 C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
+    "vr_tree_isosurface": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.POINTER(vr_options), C.c_uint32, C.c_void_p,
+                                     C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                     C.c_void_p]),
     "vr_image_ssim": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                 C.c_void_p, C.c_float, C.c_void_p]),
 }

@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <type_traits>
@@ -17,6 +18,7 @@
 
 #include "vr_build.h"
 #include "vr_frames.h"
+#include "vr_iso.h"
 #include "vr_kernels.h"
 #include "vr_normals.h"
 #include "vr_probe.h"
@@ -1081,6 +1083,56 @@ int vr_tree_build(const int32_t* cells_dev, const uint16_t* rows_dev, int64_t n,
         default: break;
     }
     *n_nodes_out = nodes;
+    return VR_OK;
+}
+
+// Marching cubes over the tree's leaf sigma on a level-`depth` lattice (kernels: vr_iso.cu, normals: vr_normals.cu).
+int vr_tree_isosurface(const vr_tree* t, int32_t depth, float level, const vr_options* opt, uint32_t flags,
+                       float* vert_dev, int64_t max_verts, uint32_t* faces_dev, int64_t max_faces, int64_t* n_verts_out,
+                       int64_t* n_faces_out, void* stream_) {
+    if (!t) return fail(VR_EINVAL, "null tree");
+    if (!n_verts_out || !n_faces_out) return fail(VR_EINVAL, "null n_verts_out or n_faces_out");
+    if (depth < 1 || depth > kIsoMaxDepth) return fail(VR_EINVAL, "depth %d outside [1, %d]", depth, kIsoMaxDepth);
+    if (!std::isfinite(level) || !(level > 0.f)) return fail(VR_EINVAL, "level %g must be finite and > 0", level);
+    if (flags & ~VR_ISO_COLOR) return fail(VR_EINVAL, "unknown flags 0x%x", flags);
+    if ((vert_dev == nullptr) != (faces_dev == nullptr))
+        return fail(VR_EINVAL, "vert_dev and faces_dev must both be NULL (count only) or both be given");
+    if (int rc = need_device(t)) return rc;
+    if (t->dev.ndc_width > 0.f) return fail(VR_EUNSUPPORTED, "isosurfaces of NDC trees are not supported");
+    const bool color = (flags & VR_ISO_COLOR) != 0;
+    if (color && coef0_only(t))
+        return fail(VR_EUNSUPPORTED, "colours unavailable for basis_dim %d (only coefficient 0 is resident)",
+                    t->dev.basis_dim);
+    int rc;
+    if ((rc = buffer_check(t, vert_dev, "vert_dev")) || (rc = buffer_check(t, faces_dev, "faces_dev"))) return rc;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    IsoArgs a{};
+    a.tree = t->dev; a.depth = depth; a.level = level; a.vert = vert_dev; a.faces = faces_dev; a.color = color;
+    if (const char* e = getenv("VR_ISO_SLAB_PLANES")) a.slab_planes = atoi(e);
+    long long nv = 0, nf = 0;
+    int launches = 0;
+    cudaError_t e = iso_run(a, false, stream, &nv, &nf, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) return cuda_fail(e, "isosurface count");
+    *n_verts_out = nv;
+    *n_faces_out = nf;
+    if (nv > INT32_MAX || nf > INT32_MAX / 3)
+        return fail(VR_EUNSUPPORTED, "the mesh has %lld vertices and %lld faces: at most %d vertices and face corners",
+                    nv, nf, INT32_MAX);
+    if (!vert_dev) return VR_OK;
+    if (max_verts < nv || max_faces < nf)
+        return fail(VR_EINVAL, "the mesh has %lld vertices and %lld faces, the outputs room for %lld and %lld", nv, nf,
+                    (long long)max_verts, (long long)max_faces);
+    launches = 0;
+    e = iso_run(a, true, stream, &nv, &nf, &launches);
+    if (e == cudaSuccess) e = normals_estimate(vert_dev, nv, faces_dev, nf, stream, &launches);
+    if (e == cudaSuccess && color) {
+        int32_t bmin, bmax;
+        basis_range(t, opt, &bmin, &bmax);
+        e = iso_color(t->dev, depth, vert_dev, nv, bmin, bmax, stream, &launches);
+    }
+    g_launches += launches;
+    if (e != cudaSuccess) return cuda_fail(e, "isosurface");
     return VR_OK;
 }
 
